@@ -21,6 +21,7 @@ import argparse
 import json
 import os
 import sys
+import tempfile
 import threading
 import time
 
@@ -30,10 +31,11 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 
 METRIC = "ChangeItems/sec on ClickBench-shaped 99-col batches (filter_rows + cast + ClickHouse native block + LZ4 frames)"
-FALLBACK_HBM_GBS = 6650.0
-
-
-TRAFFIC_PROFILE = "profiles/r2h_traffic.json"   # written by scripts/ncu_summary.py from the capture under profiles/
+FALLBACK_HBM_GBS = 3350.0     # H100 SXM data sheet (HBM3); a figure for the card, not one reached
+L2_MB = 50
+DUMP_SAMPLE = 1 << 22         # --dump-outputs: bytes drawn from the native block (16 MB of float32)
+DUMP_CHUNK = 4096             # --dump-outputs: every byte is covered by the sum of its 4 KiB chunk
+DUMP_SEED = 20240531
 
 
 def bench_config(args, ncols: int) -> dict:
@@ -49,14 +51,14 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return FALLBACK_HBM_GBS, "fallback 6.65 TB/s (B200_PROFILING.md)"
+    return FALLBACK_HBM_GBS, "fallback 3.35 TB/s (H100 SXM data sheet)"
 
 
 def make_batch(rows: int, seed: int):
-    """Seeded synthetic batch; cached under /tmp so the two arms and every N reuse one generation."""
+    """Seeded synthetic batch; cached in the temporary directory so the two arms and every N reuse one generation."""
     from transferia_b200 import abi, workload
     schema = workload.hits_schema()
-    cache = f"/tmp/tfgpu_hits_{rows}_{seed}.npz"
+    cache = os.path.join(tempfile.gettempdir(), f"tfgpu_hits_{rows}_{seed}.npz")
     if os.path.exists(cache):
         try:
             z = np.load(cache)
@@ -81,6 +83,26 @@ def make_batch(rows: int, seed: int):
     except Exception:
         pass
     return batch, schema
+
+
+def dump_outputs(eng, out_dir: str) -> None:
+    """What the timed call left on the device after its last step: the LZ4 frames a caller fetches (resident_fetch), decoded and
+    checksum-checked by the oracle's frame reader back to the native block they carry. The compressed bytes themselves are not
+    dumped: they differ run to run (DESIGN.md, Parity), the block does not. Files: stats.npy (rows out, block bytes, frames, row
+    errors, float64); block_chunk_sums.npy (byte sum of every 4 KiB chunk of the block, float64); block_sample.npy (the block's bytes
+    at DUMP_SAMPLE positions drawn with DUMP_SEED, sorted and without repeats, float32). About 17 MB for a 1 M-row step."""
+    from oracle import pyoracle as po
+    st = eng.resident_stats()
+    block, n_frames = po.ch_decode_frames(eng.resident_fetch(1, st["wire_bytes"]))
+    if block is None or len(block) != st["raw_bytes"]:
+        raise SystemExit("bench.py: the frames of the last timed step do not decode to the native block")
+    b = np.frombuffer(block, dtype=np.uint8)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "stats.npy"), np.array([st["rows_out"], len(b), n_frames, st["n_errors"]], dtype=np.float64))
+    padded = np.concatenate([b, np.zeros(-len(b) % DUMP_CHUNK, np.uint8)])
+    np.save(os.path.join(out_dir, "block_chunk_sums.npy"), padded.reshape(-1, DUMP_CHUNK).sum(axis=1, dtype=np.uint64).astype(np.float64))
+    pos = np.unique(np.random.default_rng(DUMP_SEED).integers(0, len(b), DUMP_SAMPLE)) if len(b) else np.zeros(0, np.int64)
+    np.save(os.path.join(out_dir, "block_sample.npy"), b[pos].astype(np.float32))
 
 
 class ClockSampler(threading.Thread):
@@ -228,7 +250,7 @@ def extra_paths(eng, args):
     from transferia_b200 import abi, engine, workload
     sys.path.insert(0, ROOT)
     res = {}
-    cache = f"/tmp/tf_json_lines_{args.json_lines}.bin"
+    cache = os.path.join(tempfile.gettempdir(), f"tf_json_lines_{args.json_lines}.bin")
     if os.path.exists(cache):
         text = open(cache, "rb").read(); fields = [dict(f) for f in workload.JSON_FIELDS]
     else:
@@ -279,7 +301,7 @@ def extra_paths(eng, args):
         res["debezium_emit_error"] = str(ex)
     # BASELINE configs[3]: Debezium CDC envelopes (12-field payload, schema-registry framed) -> parse -> filter_rows -> cast -> native block + LZ4
     try:
-        dcache = f"/tmp/tf_dbz_{args.dbz_msgs}.bin"
+        dcache = os.path.join(tempfile.gettempdir(), f"tf_dbz_{args.dbz_msgs}.bin")
         if os.path.exists(dcache + ".npy"):
             ddata = open(dcache, "rb").read(); dends = np.load(dcache + ".npy"); dschema_text, dtable = workload.debezium_schema_text(), ("public", "events")
         else:
@@ -313,7 +335,7 @@ def extra_paths(eng, args):
         res["debezium_parse_error"] = str(ex)
     # BASELINE configs[4]: hits-shaped CSV -> parse -> cast -> ClickHouse native block (+ LZ4)
     try:
-        ccache = f"/tmp/tf_csv_{args.csv_rows}.bin"
+        ccache = os.path.join(tempfile.gettempdir(), f"tf_csv_{args.csv_rows}.bin")
         cb, cschema = make_batch(args.csv_rows, workload.SEED)
         cschema = [dict(c, path=str(i)) for i, c in enumerate(cschema)]
         if os.path.exists(ccache):
@@ -433,6 +455,7 @@ def main():
     ap.add_argument("--e2e-mode", default="auto", choices=["auto", "one-phase", "two-phase"], help="end-to-end leg: tfgpu_push_encode (one-phase), tfgpu_push_encode_selective (two-phase), or both and report the faster (auto)")
     ap.add_argument("--gather-threads", type=int, default=0, help="host threads of the two-phase gather per pipeline (0: min(32, cores / pipelines / ranks))")
     ap.add_argument("--e2e-pipelines", type=int, default=4, help="host threads (one engine handle each) pushing batches concurrently in the end-to-end leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last one computed as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl != "reference" else args.warmup
 
@@ -502,6 +525,8 @@ def main():
     sampler.mark_end()
     launches = eng.launch_count() - l0
     ms_total = ev0.elapsed_time(ev1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(eng, args.dump_outputs)
     for kk in eng.profile_read():        # events of the LAST timed step
         kernel_ms[kk["name"]] = kernel_ms.get(kk["name"], 0.0) + kk["ms"]
     # average the dominant kernel over a few more (untimed) steps for a stable duration
@@ -597,12 +622,6 @@ def main():
         lz_bytes = st["raw_bytes"] + (st["wire_bytes"] - 25 * ((st["raw_bytes"] + args.frame_bytes - 1) // args.frame_bytes))
         achieved = lz_bytes / (lz_ms / 1e3) / 1e9 if lz_ms else 0.0
         step_ms = sum(kernel_avg.values())
-        traffic, traffic_src = None, None      # DRAM bytes per launch of the dominant kernel from the committed ncu --set full capture
-        try:
-            tj = json.load(open(os.path.join(ROOT, TRAFFIC_PROFILE)))["k_lz4_frames"]
-            traffic = int(tj["dram_bytes_read"] + tj["dram_bytes_write"]); traffic_src = TRAFFIC_PROFILE
-        except Exception:
-            pass
         out = {
             "metric": METRIC, "value": value, "unit": "rows/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms_max / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -612,7 +631,7 @@ def main():
                                "lz4_ratio_blocks_only": st["raw_bytes"] / max(1, st["wire_bytes"] - 25 * ((st["raw_bytes"] + args.frame_bytes - 1) // args.frame_bytes)),
                                "lz4_ratio_stock_liblz4_same_frames": stock_ratio,
                                "input_bytes_per_row": in_bytes / args.rows, "block_bytes_per_kept_row": st["raw_bytes"] / max(1, st["rows_out"]),
-                               "l2": "inputs larger than L2 (%.0f MB per step > 126 MB)" % (in_bytes / 1e6),
+                               "l2": "inputs larger than L2 (%.0f MB per step > %d MB)" % (in_bytes / 1e6, L2_MB),
                                "parallelism": f"dp{world} (one batch stream per GPU, its own seeded batch on every rank, no collective)", "rank": 0},
             "clocks": sampler.result(),
             "e2e": {"value": e2e_value, "unit": "rows/s", "h2d_bytes_per_step": int(h2d_bytes), "d2h_bytes_per_step": d2h, "host_layout": args.host_layout, "host_buffers": args.host_buffers, "numa_node": numa,
@@ -621,7 +640,7 @@ def main():
                     "steps": e2e_steps, "pipelines": P, "timing": "host wall clock over synchronous calls (tfgpu_push_encode / tfgpu_push_encode_selective over pinned host columns; H2D counted by the engine)"},
             "gpu_launches": int(launches),
             "roofline": {"bound": "hbm", "kernel": "k_lz4_frames", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak if peak else None, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                         "frac": achieved / peak if peak else None, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": int(lz_bytes), "kernel_ms": lz_ms,
                          "kernel_share_of_step": lz_ms / step_ms if step_ms else None,
                          "kernel_share_basis": "sum of the per-kernel CUDA-event times (as in the serialised ncu launch list); k_frame_seal overlaps the next step on a side stream, so that sum exceeds ms_per_step",

@@ -2,7 +2,7 @@
  * filter_rows + cast + ClickHouse native block + LZ4 frames on the GPU -> one INSERT over the native protocol.
  *   gcc -std=c99 -Iinclude examples/push_clickhouse.c -Ltransferia_b200 -ltfgpu -o push_clickhouse
  *   LD_LIBRARY_PATH=transferia_b200 ./push_clickhouse 127.0.0.1 9000
- * (the test suite only compiles and links it; running it needs a B200 and a ClickHouse server) */
+ * (the test suite only compiles and links it; running it needs an H100 and a ClickHouse server) */
 #include <arpa/inet.h>
 #include <netinet/in.h>
 #include <stdio.h>

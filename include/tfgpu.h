@@ -1,5 +1,5 @@
 /*
- * tfgpu.h — C-ABI of the B200 columnar transform engine.
+ * tfgpu.h — C-ABI of the H100 columnar transform engine.
  *
  * This is the drop-in boundary for ONE hot path of transferia/transferia:
  *
@@ -424,7 +424,7 @@ uint64_t tfgpu_engine_launch_count(const tfgpu_engine* e);
 int tfgpu_profile_enable(tfgpu_engine* e, int on);
 const char* tfgpu_profile_read(tfgpu_engine* e);
 
-/* Library identity: "tfgpu <version> sm_100a". */
+/* Library identity: "tfgpu <version> sm_90a". */
 const char* tfgpu_version(void);
 
 #ifdef __cplusplus

@@ -1,4 +1,4 @@
-// Device-visible descriptors shared by all kernels (sm_100a).
+// Device-visible descriptors shared by all kernels (sm_90a).
 #pragma once
 #include <cstdint>
 #include "../../include/tfgpu.h"

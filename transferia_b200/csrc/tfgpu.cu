@@ -1,5 +1,5 @@
-// C-ABI of the B200 columnar transform engine (include/tfgpu.h). Host orchestration only: every
-// per-row operation runs in the sm_100a kernels of kernels_*.cuh.  There is no CPU fallback: without
+// C-ABI of the H100 columnar transform engine (include/tfgpu.h). Host orchestration only: every
+// per-row operation runs in the sm_90a kernels of kernels_*.cuh.  There is no CPU fallback: without
 // a CUDA device tfgpu_engine_create fails with TF_E_FATAL_NODEVICE.
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -69,7 +69,7 @@ struct tfgpu_engine {
     std::string last_error;
     uint64_t launches = 0;
     uint32_t frame_bytes = LZ_MAX_FRAME;
-    int sm_count = 148;
+    int sm_count = 132;                 // H100 SXM; replaced by the device's count in tfgpu_engine_create
     std::vector<std::unique_ptr<PlanDev>> plans;
     // arenas
     DevBuf in_arena, work, raw, slots, wire, strict_stage, lens_arena, lens_arena2, csv_text, csv_stage, json_msgs, n2f_stage, n2f_heap, off_scratch;
@@ -429,7 +429,7 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
     const uint32_t* sel = (has_filter && n) ? e->sel : nullptr;
     const uint32_t ntiles = (uint32_t)((n + TF_STR_TILE - 1) / TF_STR_TILE);
     // (the string kernels keep one CTA per tile group and exit early past the kept rows: a capped grid with a stride loop
-    // makes the CTAs of the heavy columns run several groups back to back; measured 0.18 -> 0.25 ms on the headline batch)
+    // makes the CTAs of the heavy columns run several groups back to back, which measured slower on the headline batch)
     const uint32_t str_gx = std::max(1u, (ntiles + TF_STR_GROUP - 1) / TF_STR_GROUP);
     EncodeArgs ea{e->d_cols, pd.d_str_slots, sel, e->d_state, e->raw.p, e->tile_sum, e->tile_base, sz.ntiles_cap, columnar ? 1 : 0};
     if (!has_filter || !n) {
@@ -471,7 +471,7 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
         e->prof_begin("k_layout_finish", s); launch_k_layout_finish(1, 256, 0, s, la); e->prof_end(s);
         if (n) {
             // (the fixed-width streams and the String columns write disjoint parts of the block, but running them on two streams
-            // was measured slower: both are latency-bound gathers that already fill the SMs: 0.087 + 0.182 ms in sequence, 0.30 ms side by side)
+            // was measured slower than running them in sequence: both are latency-bound gathers that already fill the SMs)
             if (pd.n_fixed_slots) {
                 // widest stream is 8 bytes per row: words = 2n (+1 for misalignment)
                 const uint32_t gx = grid_cap(e, (uint32_t)((2 * n + 2 + TF_FIX_TILE_WORDS - 1) / TF_FIX_TILE_WORDS), (uint32_t)pd.n_fixed_slots, 6);
@@ -550,7 +550,7 @@ static bool wire_known(int wire_fmt) { return wire_fmt == TF_WIRE_CH_NATIVE || w
 
 extern "C" {
 
-const char* tfgpu_version(void) { return "tfgpu 0.1.0 sm_100a"; }
+const char* tfgpu_version(void) { return "tfgpu 0.1.0 sm_90a"; }
 
 int tfgpu_engine_create(const char* cfg_json, const int* device_ids, int n_devices, tfgpu_engine** out) {
     if (!out) return TF_E_FATAL_ARG;

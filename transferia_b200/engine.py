@@ -6,7 +6,7 @@
                                                                         providers/clickhouse/sink_table.go:605-704
     PushResult.errors       ~ TransformerResult.Errors                  pkg/abstract/transformer.go:40-48
 
-Everything computes in libtfgpu.so (hand-written sm_100a kernels).  There is NO CPU fallback: if the
+Everything computes in libtfgpu.so (hand-written sm_90a kernels).  There is NO CPU fallback: if the
 library is missing or no CUDA device is present, construction raises.
 """
 from __future__ import annotations
