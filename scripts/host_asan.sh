@@ -1,49 +1,38 @@
 #!/bin/bash
-# Host-side C++ (row transposer, sink push / dispatcher, ClickHouse writer) under AddressSanitizer + UBSan: the three host translation units are
-# built with g++ into a library of their own, the device entry points of tfgpu.h are stubbed (they answer TF_E_FATAL_NODEVICE), and the CPU tests
-# that drive the host code (fuzzers included) run against it; tfgpu_plan_validate is the real one (plan.hpp: plan builder + filter grammar).
+# Host-side C++ (row transposer, sink push / dispatcher, ClickHouse writer, plan validation and queue batchers) under AddressSanitizer + UBSan:
+# the four host translation units are built with g++ into a library of their own, the device entry points of tfgpu.h are stubbed (they answer
+# TF_E_FATAL_NODEVICE), and the CPU tests that drive the host code (fuzzers included) run against it.
 set -e
 ROOT=$(cd "$(dirname "$0")/.." && pwd); OUT=${1:-/tmp/tfhost_asan}; mkdir -p "$OUT"
-python - "$ROOT" "$OUT" <<'PY'
+CSRC="$ROOT/transferia_b200/csrc"
+HOST_TUS=("$CSRC/host_rows.cu" "$CSRC/host_sink.cu" "$CSRC/host_chwire.cu" "$CSRC/host_plan.cu")
+python - "$ROOT" "$OUT" "$CSRC/host_plan.cu" <<'PY'
 import re, sys
-root, out = sys.argv[1], sys.argv[2]
+root, out, host_plan = sys.argv[1], sys.argv[2], sys.argv[3]
 hdr = re.sub(r"/\*.*?\*/", "", open(root + "/include/tfgpu.h").read(), flags=re.S)
 protos = re.findall(r"^\s*((?:const\s+)?[\w]+(?:\s*\*)?)\s+(tfgpu_\w+)\s*\(([^;{]*?)\)\s*;", hdr, flags=re.M | re.S)
+real = set(re.findall(r"^int (tfgpu_\w+)\(", open(host_plan).read(), flags=re.M))     # defined by host_plan.cu, compiled below
 lines = ['#include "%s/include/tfgpu.h"' % root, 'extern "C" {']
 for ret, name, args in protos:
-    if name == "tfgpu_plan_validate":
-        continue                                   # the real one: plan.hpp is host C++ (see below)
+    if name in real:
+        continue
     ret = ret.strip(); body = "{}" if ret == "void" else ("{ return TF_E_FATAL_NODEVICE; }" if ret == "int" else "{ return 0; }")
     lines.append("%s %s(%s) %s" % (ret, name, " ".join(args.split()), body))
 open(out + "/stubs.cpp", "w").write("\n".join(lines) + "\n}\n")
-# tfgpu_plan_validate as tfgpu.cu defines it, over the same plan.hpp (the plan builder and the filter grammar are host code)
-open(out + "/plan_validate.cpp", "w").write('''#include <cstring>
-#include "%s/transferia_b200/csrc/plan.hpp"
-extern "C" int tfgpu_plan_validate(const char* ns, const char* name, const char* schema_json, const char* transformers_json, const char* sink_json,
-                                   char* describe_out, uint64_t cap, char* err_out, uint64_t err_cap) {
-    auto put = [](char* dst, uint64_t cap_, const std::string& s) { if (dst && cap_) { size_t n = s.size() < cap_ - 1 ? s.size() : cap_ - 1; std::memcpy(dst, s.data(), n); dst[n] = 0; } };
-    if (!schema_json || !name) return TF_E_FATAL_ARG;
-    try {
-        tfplan::Plan pl = tfplan::build_plan(ns ? ns : "", name, schema_json, transformers_json ? transformers_json : "", sink_json ? sink_json : "");
-        if (describe_out && pl.describe.size() + 1 > cap) { put(err_out, err_cap, "describe buffer too small"); return TF_E_FATAL_ARG; }
-        put(describe_out, cap, pl.describe);
-        return TF_OK;
-    } catch (const tfplan::FatalError& f) { put(err_out, err_cap, f.what()); return f.code; }
-    catch (const std::exception& x) { put(err_out, err_cap, x.what()); return TF_E_FATAL_CONFIG; }
-}
-''' % root)
 PY
 g++ -std=c++17 -O1 -g -fsanitize=address,undefined -fno-omit-frame-pointer -fPIC -shared -I/usr/local/cuda/include \
-    -x c++ "$ROOT/transferia_b200/csrc/host_rows.cu" "$ROOT/transferia_b200/csrc/host_sink.cu" "$ROOT/transferia_b200/csrc/host_chwire.cu" "$OUT/stubs.cpp" "$OUT/plan_validate.cpp" \
-    -o "$OUT/libtfhost_asan.so" -L/usr/local/cuda/lib64 -lcudart
+    -x c++ "${HOST_TUS[@]}" "$OUT/stubs.cpp" -o "$OUT/libtfhost_asan.so" -L/usr/local/cuda/lib64 -lcudart
 cd "$ROOT"
 TFGPU_LIB_PATH="$OUT/libtfhost_asan.so" LD_PRELOAD="$(gcc -print-file-name=libasan.so) $(gcc -print-file-name=libubsan.so)" \
     ASAN_OPTIONS=detect_leaks=0:halt_on_error=1 UBSAN_OPTIONS=print_stacktrace=1:halt_on_error=1 \
     python -m pytest tests/test_rows.py tests/test_sink_push.py tests/test_ch_wire.py tests/test_host_cpu.py tests/test_regex_replace.py -q -m "not gpu" -p no:cacheprovider \
-    -k "not exports and not sm100a and not no_cpu_fallback and not gloo and not bench_reference and not c_example"
+    -k "not exports and not sm90a and not no_cpu_fallback and not gloo and not bench_reference and not c_example"
+# the queue serializer batchers (host_plan.cu)
+TFGPU_LIB_PATH="$OUT/libtfhost_asan.so" LD_PRELOAD="$(gcc -print-file-name=libasan.so) $(gcc -print-file-name=libubsan.so)" \
+    ASAN_OPTIONS=detect_leaks=0:halt_on_error=1 UBSAN_OPTIONS=print_stacktrace=1:halt_on_error=1 \
+    python -m pytest tests/test_serializers.py tests/test_debezium_emit.py -q -m "not gpu" -p no:cacheprovider -k "queue_json_batching or queue_debezium_batching"
 # the threaded parts (worker pool of the transposer / gather / column-wise replace, dispatcher lanes and its delivery gate) under ThreadSanitizer
 g++ -std=c++17 -O1 -g -fsanitize=thread -fno-omit-frame-pointer -fPIC -shared -I/usr/local/cuda/include \
-    -x c++ "$ROOT/transferia_b200/csrc/host_rows.cu" "$ROOT/transferia_b200/csrc/host_sink.cu" "$ROOT/transferia_b200/csrc/host_chwire.cu" "$OUT/stubs.cpp" "$OUT/plan_validate.cpp" \
-    -o "$OUT/libtfhost_tsan.so" -L/usr/local/cuda/lib64 -lcudart
+    -x c++ "${HOST_TUS[@]}" "$OUT/stubs.cpp" -o "$OUT/libtfhost_tsan.so" -L/usr/local/cuda/lib64 -lcudart
 TFGPU_LIB_PATH="$OUT/libtfhost_tsan.so" LD_PRELOAD="$(gcc -print-file-name=libtsan.so)" TSAN_OPTIONS="halt_on_error=1 report_signal_unsafe=0" \
     python -m pytest tests/test_rows.py tests/test_sink_push.py tests/test_regex_replace.py -q -m "not gpu" -p no:cacheprovider -k "dispatcher or two_pools or host_gather or transposer_fuzz or strict_single or replace_steps or mixed_text or inverse_transposer or under_the_dispatcher"

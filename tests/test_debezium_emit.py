@@ -15,6 +15,7 @@ from transferia_b200 import abi
 
 G = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "debezium_emit_goldens.json"), encoding="utf-8"))
 OPTS = {"ignore_unknown_sources": True, "version": "1.1.2.Final", "topic_prefix": "fullfillment", "database": "pguser", "source_type": "pg"}
+TF_E_FATAL_CONFIG, TF_E_FATAL_UNSUPPORTED = -1, -2          # include/tfgpu.h
 
 
 def _golden_batch():
@@ -307,12 +308,14 @@ def test_product_host_template_matches_oracle(po):
             assert key_end == int(ks[0]), (st, extra)
     # refusals decided on the host: errUnknownSource, types and (type, column type) pairs left to Go, rewritten pg columns, bad options
     ok = {"name": "i", "type": "int32", "key": True, "original_type": "pg:integer"}
-    for sch, trs, opts in (([{"name": "i", "type": "int32"}], [], {"version": "1"}),
-                           ([dict(ok, original_type="pg:interval")], [], OPTS), ([dict(ok, original_type="pg:bigint")], [], OPTS), ([dict(ok, original_type="mysql:int(11)")], [], OPTS),
-                           ([ok], [{"convert_to_string": {}}], OPTS), ([ok], [{"mask_field": {"columns": ["i"], "maskFunctionHash": {"userDefinedSalt": "s"}}}], {"version": "1"}),
-                           ([ok], [], dict(OPTS, source_type="oracle"))):
-        with pytest.raises(engine.EngineError):
+    for sch, trs, opts, rc in (([{"name": "i", "type": "int32"}], [], {"version": "1"}, TF_E_FATAL_CONFIG),
+                               ([dict(ok, original_type="pg:interval")], [], OPTS, TF_E_FATAL_UNSUPPORTED), ([dict(ok, original_type="pg:bigint")], [], OPTS, TF_E_FATAL_UNSUPPORTED),
+                               ([dict(ok, original_type="mysql:int(11)")], [], OPTS, TF_E_FATAL_UNSUPPORTED), ([ok], [{"convert_to_string": {}}], OPTS, TF_E_FATAL_UNSUPPORTED),
+                               ([ok], [{"mask_field": {"columns": ["i"], "maskFunctionHash": {"userDefinedSalt": "s"}}}], {"version": "1"}, TF_E_FATAL_CONFIG),
+                               ([ok], [], dict(OPTS, source_type="oracle"), TF_E_FATAL_UNSUPPORTED)):
+        with pytest.raises(engine.EngineError) as ei:
             engine.emit_debezium_validate("s", "t", sch, trs, opts)
+        assert ei.value.rc == rc, (sch, trs, opts)
     # a masked pg column loses its original type (hmac_hasher.go:41): common path, needs ignore_unknown_sources
     d = engine.emit_debezium_validate("s", "t", [ok], [{"mask_field": {"columns": ["i"], "maskFunctionHash": {"userDefinedSalt": "s"}}}], OPTS)
     assert d["forms"] == [0]
@@ -393,17 +396,21 @@ def test_device_emitter_all_types_and_resident(eng, po):
 def test_device_emitter_refusals(eng):
     from transferia_b200.engine import EngineError
     b = abi.Batch(1, [abi.fixed_to_column(abi.TF_INT32, [1])])
+    # each refusal has the code emit_debezium_validate gives it: UNSUPPORTED keeps the table on the Go emitter
     pid = eng.plan("s", "t", [{"name": "i", "type": "int32", "key": True}], [])
-    with pytest.raises(EngineError):        # errUnknownSource (emitter_value_converter.go:183-191)
+    with pytest.raises(EngineError) as ei:        # errUnknownSource (emitter_value_converter.go:183-191)
         eng.emit_debezium(pid, b, {"version": "1"})
+    assert ei.value.rc == TF_E_FATAL_CONFIG
     for col in ({"name": "i", "type": "int32", "key": True, "original_type": "pg:interval"}, {"name": "i", "type": "int32", "key": True, "original_type": "pg:bigint"},
                 {"name": "i", "type": "int32", "key": True, "original_type": "mysql:int(11)"}):
         pid = eng.plan("s", "t", [col], [])
-        with pytest.raises(EngineError):
+        with pytest.raises(EngineError) as ei:
             eng.emit_debezium(pid, b, OPTS)
+        assert ei.value.rc == TF_E_FATAL_UNSUPPORTED, col
     pid = eng.plan("s", "t", [{"name": "i", "type": "int32", "key": True, "original_type": "pg:integer"}], [{"convert_to_string": {}}])
-    with pytest.raises(EngineError):        # a transformer rewrote a pg-typed column: AddPg would reject the value
+    with pytest.raises(EngineError) as ei:        # a transformer rewrote a pg-typed column: AddPg would reject the value
         eng.emit_debezium(pid, b, OPTS)
+    assert ei.value.rc == TF_E_FATAL_UNSUPPORTED
 
 
 # ----------------------------------------------------------------------------------------------------------- update / delete events

@@ -335,15 +335,19 @@ def test_full_size_batch_properties(eng, po):
 def test_api_errors(eng):
     schema = [{"name": "a", "type": "int32", "required": True}]
     pid = eng.plan("db", "t", schema, [], {"type": "clickhouse"})
+    unsupported, arg = -2, -3                    # TF_E_FATAL_UNSUPPORTED, TF_E_FATAL_ARG (include/tfgpu.h)
     with pytest.raises(engine.EngineError) as ei:
         eng.push_encode(pid, abi.Batch(1, [abi.fixed_to_column(abi.TF_INT32, [1]), abi.fixed_to_column(abi.TF_INT32, [1])]), RAW)
-    assert ei.value.rc < 0
-    with pytest.raises(engine.EngineError):      # a text value in an int32 column is not strictified on the device (an int64 value is: test_device_strictify_loose_value_types)
+    assert ei.value.rc == arg
+    with pytest.raises(engine.EngineError) as ei:      # a text value in an int32 column is not strictified on the device (an int64 value is: test_device_strictify_loose_value_types)
         eng.push_encode(pid, abi.Batch(1, [abi.strings_to_column(abi.TF_UTF8, [b"1"])]), RAW)
-    with pytest.raises(engine.EngineError):
+    assert ei.value.rc == arg
+    with pytest.raises(engine.EngineError) as ei:
         eng.plan("db", "t", schema, [{"mask_field": {"columns": ["a"], "maskFunctionHash": {"userDefinedSalt": "s"}}}, {"filter_rows": {"filter": "a = 'x'"}}], {"type": "clickhouse"})
-    with pytest.raises(engine.EngineError):
+    assert ei.value.rc == unsupported
+    with pytest.raises(engine.EngineError) as ei:
         eng.push_encode(pid, abi.Batch(1, [abi.fixed_to_column(abi.TF_INT32, [1])]), 99)          # unknown wire format
+    assert ei.value.rc == unsupported
 
 
 def assert_batches_equal(a: abi.Batch, b: abi.Batch):

@@ -16,6 +16,7 @@
 #include "plan.hpp"
 #include "device_types.cuh"
 #include "launch.hpp"
+#include "host_internal.hpp"
 
 using namespace tfk;
 
@@ -26,15 +27,28 @@ struct CudaError { cudaError_t e; const char* what; };
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// Grow-only device buffer, freed with its owner.
 struct DevBuf {
     uint8_t* p = nullptr; size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
     void ensure(size_t n) {
         if (n <= cap) return;
         if (p) { CK(cudaDeviceSynchronize()); CK(cudaFree(p)); p = nullptr; cap = 0; }
         size_t want = align_up(n + n / 8 + 4096, 1 << 20);
         CK(cudaMalloc(&p, want)); cap = want;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+};
+
+// Offsets of the buffers carved out of one arena, in order: each starts on a 256-byte boundary. `slack` bytes past the end of
+// each buffer stay inside its slot: the string kernels' 16-byte loads may read that far. An empty buffer still takes a slot.
+struct Layout {
+    size_t slack, end = 0;
+    explicit Layout(size_t slack_ = 0) : slack(slack_) {}
+    size_t take(size_t bytes) { const size_t at = end; end += align_up(std::max<size_t>(bytes + slack, 1), 256); return at; }
+    size_t total() const { return end; }
 };
 
 struct PlanDev {
@@ -59,12 +73,13 @@ struct PlanDev {
 
 struct tfgpu_engine {
     int device = 0;
-    cudaStream_t own_stream = nullptr, stream = nullptr, side_stream = nullptr;   // side_stream: string encode runs beside the fixed-width encode
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-    // The checksum chain and the wire gather of an LZ4 batch run on two side streams and are NOT joined at the end of the call: the
-    // next batch's filter / encode kernels overlap them (they only wait before they reuse the frame slots). join_tail() orders the
-    // main stream after them; every path that reads results, changes layout or leaves the LZ4 format calls it.
-    cudaStream_t side2_stream = nullptr; cudaEvent_t ev_tail2 = nullptr; bool tail_pending = false; uint64_t tail_nrows = 0, tail_nframes_max = 0; const void* tail_plan = nullptr;
+    cudaStream_t own_stream = nullptr, stream = nullptr;
+    // The checksum kernel (k_frame_seal) of an LZ4 batch runs on side_stream and is NOT joined at the end of the call: the next
+    // batch's filter / encode kernels overlap it (its k_lz4_frames waits first, as it rewrites the wire bytes and frame sizes the
+    // checksum reads). join_tail() orders the main stream after it; every path that reads results, changes layout or leaves the
+    // LZ4 format calls it.
+    cudaStream_t side_stream = nullptr; cudaEvent_t ev_fork = nullptr, ev_tail = nullptr;
+    bool tail_pending = false; uint64_t tail_nrows = 0, tail_nframes_max = 0; const void* tail_plan = nullptr;
     uint64_t* d_tail = nullptr;
     std::string last_error;
     uint64_t launches = 0;
@@ -72,7 +87,7 @@ struct tfgpu_engine {
     int sm_count = 132;                 // H100 SXM; replaced by the device's count in tfgpu_engine_create
     std::vector<std::unique_ptr<PlanDev>> plans;
     // arenas
-    DevBuf in_arena, work, raw, slots, wire, strict_stage, lens_arena, lens_arena2, csv_text, csv_stage, json_msgs, n2f_stage, n2f_heap, off_scratch;
+    DevBuf in_arena, work, raw, wire, strict_stage, lens_arena, lens_arena2, csv_text, csv_stage, json_msgs, n2f_stage, n2f_heap, off_scratch;
     DState* d_state = nullptr; DCol* d_cols = nullptr; size_t d_cols_cap = 0;
     int32_t* d_call_slots = nullptr; ColRegions* d_regions = nullptr; size_t d_call_cap = 0;   // columnar mode, per call
     // pointers into `work` for the last call
@@ -119,7 +134,7 @@ namespace {
 
 void join_tail(tfgpu_engine* e) {
     if (!e->tail_pending) return;
-    CK(cudaStreamWaitEvent(e->stream, e->ev_tail2, 0));
+    CK(cudaStreamWaitEvent(e->stream, e->ev_tail, 0));
     e->tail_pending = false;
 }
 int fail(tfgpu_engine* e, int code, const std::string& msg) { if (e) e->last_error = msg; return code; }
@@ -129,28 +144,22 @@ int cuda_fail(tfgpu_engine* e, const CudaError& c) {
     return fail(e, c.e == cudaErrorMemoryAllocation ? TF_E_RETRY_OOM : TF_E_RETRY_LAUNCH, m);
 }
 
-// encoding/json appendString with escapeHTML off, for column names (json.go:56-58)
-std::string host_json_quote_nohtml(const std::string& in) {
-    static const char* hex = "0123456789abcdef";
-    std::string d = "\""; const uint8_t* s = (const uint8_t*)in.data(); const size_t n = in.size();
-    for (size_t i = 0; i < n;) {
-        const uint8_t b = s[i];
-        if (b < 0x80) {
-            if (b >= 0x20 && b != '"' && b != '\\') d += (char)b;
-            else { d += '\\'; switch (b) { case '"': case '\\': d += (char)b; break; case '\b': d += 'b'; break; case '\f': d += 'f'; break; case '\n': d += 'n'; break; case '\r': d += 'r'; break; case '\t': d += 't'; break;
-                                            default: d += "u00"; d += hex[b >> 4]; d += hex[b & 15]; } }
-            i++; continue;
-        }
-        uint32_t r = 0xFFFD; size_t w = 1;
-        if (b >= 0xC2 && b <= 0xDF && i + 1 < n && (s[i + 1] & 0xC0) == 0x80) { r = ((b & 0x1Fu) << 6) | (s[i + 1] & 0x3Fu); w = 2; }
-        else if (b >= 0xE0 && b <= 0xEF && i + 2 < n && (s[i + 1] & 0xC0) == 0x80 && (s[i + 2] & 0xC0) == 0x80) { const uint32_t t = ((b & 0x0Fu) << 12) | ((s[i + 1] & 0x3Fu) << 6) | (s[i + 2] & 0x3Fu); if (t >= 0x800 && !(t >= 0xD800 && t <= 0xDFFF)) { r = t; w = 3; } }
-        else if (b >= 0xF0 && b <= 0xF4 && i + 3 < n && (s[i + 1] & 0xC0) == 0x80 && (s[i + 2] & 0xC0) == 0x80 && (s[i + 3] & 0xC0) == 0x80) { const uint32_t t = ((b & 0x07u) << 18) | ((s[i + 1] & 0x3Fu) << 12) | ((s[i + 2] & 0x3Fu) << 6) | (s[i + 3] & 0x3Fu); if (t >= 0x10000 && t <= 0x10FFFF) { r = t; w = 4; } }
-        if (r == 0xFFFD && w == 1) d += "\\ufffd";
-        else if (r == 0x2028 || r == 0x2029) { d += "\\u202"; d += hex[r & 0xF]; }
-        else d.append((const char*)s + i, w);
-        i += w;
-    }
-    return d + "\"";
+// The exception boundary of every entry point that takes an engine: selects its device, runs `body` (which returns a TF_* code)
+// and turns what it throws into a code, with the message in e->last_error. Nothing crosses extern "C".
+template <typename F> int on_device(tfgpu_engine* e, F&& body) {
+    try {
+        CK(cudaSetDevice(e->device));
+        return body();
+    } catch (const tfplan::FatalError& f) { return fail(e, f.code, f.what()); }
+    catch (const CudaError& c) { return cuda_fail(e, c); }
+    catch (const std::bad_alloc&) { return fail(e, TF_E_RETRY_OOM, "host allocation failed"); }
+    catch (const std::exception& x) { return fail(e, TF_E_FATAL_CONFIG, x.what()); }
+}
+
+// malformed opts_json is a configuration error that names the argument
+tfj::ValuePtr parse_opts_json(const char* js) {
+    try { return tfj::parse(js); }
+    catch (const std::runtime_error& x) { throw tfplan::FatalError(TF_E_FATAL_CONFIG, std::string("opts_json: ") + x.what()); }
 }
 
 int in_width(int tf) {
@@ -163,9 +172,14 @@ int in_width(int tf) {
     return 0;
 }
 
-template <typename T> T* carve(uint8_t*& p, size_t count) { T* r = (T*)p; p += align_up(count * sizeof(T), 256); return r; }
+// Host image of a block of device constants, laid out by a Layout; copied to the device in one transfer.
+struct ConstImage {
+    Layout L; std::vector<uint8_t> bytes;
+    size_t add(const void* src, size_t n) { const size_t at = L.take(n); bytes.resize(L.total()); if (n) std::memcpy(bytes.data() + at, src, n); return at; }
+    uint8_t* upload(DevBuf& dst) { dst.ensure(bytes.size()); CK(cudaMemcpy(dst.p, bytes.data(), bytes.size(), cudaMemcpyHostToDevice)); return dst.p; }
+};
 
-void upload_plan(tfgpu_engine* e, PlanDev& pd) {
+void upload_plan(PlanDev& pd) {
     const tfplan::Plan& pl = pd.plan;
     const size_t nc = pl.in_schema.size();
     // which mask step (if any) owns each column
@@ -244,33 +258,24 @@ void upload_plan(tfgpu_engine* e, PlanDev& pd) {
     }
     pd.n_fsteps = (int)fsteps.size(); pd.n_fixed_slots = (int)pd.fixed_slots.size(); pd.n_str = (int)pd.str_slots.size(); pd.n_mask_cols = (int)pd.mask_slot_cols.size();
     pd.n_tostr = 0; for (size_t c = 0; c < pd.col_out_kind.size(); c++) if (pd.col_out_kind[c] == OK_TOSTR) pd.n_tostr++;
-    size_t total = 0;
-    auto need = [&](size_t n) { total += align_up(n ? n : 1, 256); };
-    need(terms.size() * sizeof(DTerm)); need(expr_off.size() * 4); need(fsteps.size() * sizeof(DFilterStep)); need(pl.blob.size());
-    need(pl.col_headers.size()); need(pl.col_header_off.size() * 4); need(pd.fixed_slots.size() * 4); need(pd.str_slots.size() * 4);
-    need(pd.mask_slot_cols.size() * 4); need(keys.size() * sizeof(MaskKey)); need(pl.out_cols.size() * 4); need(jcols.size() * sizeof(JsonCol)); need(jnames.size());
-    need(sjcols.size() * sizeof(JsonCol)); need(scsvcols.size() * sizeof(JsonCol)); need(snames.size());
     std::vector<ShardCol> shcols;
     for (size_t k = 0; k < pl.shard_cols.size(); k++) shcols.push_back(ShardCol{pl.shard_cols[k], pl.shard_form[k], 0, 0});
-    need(shcols.size() * sizeof(ShardCol));
-    pd.consts.ensure(total);
-    uint8_t* p = pd.consts.p;
-    auto put = [&](const void* src, size_t n) { uint8_t* d = p; if (n) CK(cudaMemcpy(d, src, n, cudaMemcpyHostToDevice)); p += align_up(n ? n : 1, 256); return d; };
-    pd.d_terms = (DTerm*)put(terms.data(), terms.size() * sizeof(DTerm));
-    pd.d_expr_off = (uint32_t*)put(expr_off.data(), expr_off.size() * 4);
-    pd.d_fsteps = (DFilterStep*)put(fsteps.data(), fsteps.size() * sizeof(DFilterStep));
-    pd.d_blob = put(pl.blob.data(), pl.blob.size());
-    pd.d_col_headers = put(pl.col_headers.data(), pl.col_headers.size());
-    pd.d_col_header_off = (uint32_t*)put(pl.col_header_off.data(), pl.col_header_off.size() * 4);
-    pd.d_fixed_slots = (int32_t*)put(pd.fixed_slots.data(), pd.fixed_slots.size() * 4);
-    pd.d_str_slots = (int32_t*)put(pd.str_slots.data(), pd.str_slots.size() * 4);
-    pd.d_mask_slots = (int32_t*)put(pd.mask_slot_cols.data(), pd.mask_slot_cols.size() * 4);
-    pd.d_mask_keys = (MaskKey*)put(keys.data(), keys.size() * sizeof(MaskKey));
-    { std::vector<int32_t> oc(pl.out_cols.begin(), pl.out_cols.end()); pd.d_out_cols = (int32_t*)put(oc.data(), oc.size() * 4); }
-    pd.d_jcols = (JsonCol*)put(jcols.data(), jcols.size() * sizeof(JsonCol)); pd.d_jnames = put(jnames.data(), jnames.size());
-    pd.d_sjcols = (JsonCol*)put(sjcols.data(), sjcols.size() * sizeof(JsonCol)); pd.d_scsvcols = (JsonCol*)put(scsvcols.data(), scsvcols.size() * sizeof(JsonCol)); pd.d_snames = put(snames.data(), snames.size());
-    pd.d_shard_cols = (ShardCol*)put(shcols.data(), shcols.size() * sizeof(ShardCol));
-    (void)e;
+    const std::vector<int32_t> oc(pl.out_cols.begin(), pl.out_cols.end());
+    ConstImage ci;
+    const size_t o_terms = ci.add(terms.data(), terms.size() * sizeof(DTerm)), o_expr_off = ci.add(expr_off.data(), expr_off.size() * 4),
+                 o_fsteps = ci.add(fsteps.data(), fsteps.size() * sizeof(DFilterStep)), o_blob = ci.add(pl.blob.data(), pl.blob.size()),
+                 o_hdr = ci.add(pl.col_headers.data(), pl.col_headers.size()), o_hdr_off = ci.add(pl.col_header_off.data(), pl.col_header_off.size() * 4),
+                 o_fixed = ci.add(pd.fixed_slots.data(), pd.fixed_slots.size() * 4), o_str = ci.add(pd.str_slots.data(), pd.str_slots.size() * 4),
+                 o_mask = ci.add(pd.mask_slot_cols.data(), pd.mask_slot_cols.size() * 4), o_keys = ci.add(keys.data(), keys.size() * sizeof(MaskKey)),
+                 o_out = ci.add(oc.data(), oc.size() * 4), o_jcols = ci.add(jcols.data(), jcols.size() * sizeof(JsonCol)), o_jnames = ci.add(jnames.data(), jnames.size()),
+                 o_sjcols = ci.add(sjcols.data(), sjcols.size() * sizeof(JsonCol)), o_scsv = ci.add(scsvcols.data(), scsvcols.size() * sizeof(JsonCol)),
+                 o_snames = ci.add(snames.data(), snames.size()), o_shard = ci.add(shcols.data(), shcols.size() * sizeof(ShardCol));
+    uint8_t* P = ci.upload(pd.consts);
+    pd.d_terms = (DTerm*)(P + o_terms); pd.d_expr_off = (uint32_t*)(P + o_expr_off); pd.d_fsteps = (DFilterStep*)(P + o_fsteps); pd.d_blob = P + o_blob;
+    pd.d_col_headers = P + o_hdr; pd.d_col_header_off = (uint32_t*)(P + o_hdr_off);
+    pd.d_fixed_slots = (int32_t*)(P + o_fixed); pd.d_str_slots = (int32_t*)(P + o_str); pd.d_mask_slots = (int32_t*)(P + o_mask); pd.d_mask_keys = (MaskKey*)(P + o_keys);
+    pd.d_out_cols = (int32_t*)(P + o_out); pd.d_jcols = (JsonCol*)(P + o_jcols); pd.d_jnames = P + o_jnames;
+    pd.d_sjcols = (JsonCol*)(P + o_sjcols); pd.d_scsvcols = (JsonCol*)(P + o_scsv); pd.d_snames = P + o_snames; pd.d_shard_cols = (ShardCol*)(P + o_shard);
 }
 
 struct Sizes { uint64_t raw_bound, n_frames_max, wire_bound; uint32_t ntiles_cap, nblocks; };
@@ -309,6 +314,37 @@ static void launch_offsets(tfgpu_engine* e, const uint32_t* d_len, uint64_t nrow
     e->prof_begin("k_offsets_write", s); launch_k_offsets_write(dim3(nchunks, nslots), 1024, 0, s, d_len, nrows, nchunks, cs, d_tot, d_off); e->prof_end(s);
 }
 
+// Text heaps of k var-width columns whose cell lengths are d_len [k][nrows]: offsets d_off [k][nrows+1] and totals d_tot [k] on the
+// device, then every column's heap at a 16-byte-aligned base inside `heap` (bases uploaded to d_base [k]). Offsets are uint32, so a
+// column of 4 GiB or more is refused with `too_big`.
+struct Heaps { std::vector<uint64_t> total, base; };
+Heaps size_heaps(tfgpu_engine* e, const uint32_t* d_len, uint64_t nrows, uint32_t k, uint32_t* d_off, uint64_t* d_tot, uint64_t* d_base,
+                 DevBuf& heap, const char* too_big) {
+    cudaStream_t s = e->stream;
+    launch_offsets(e, d_len, nrows, k, d_off, d_tot, s);
+    Heaps h{std::vector<uint64_t>(k), std::vector<uint64_t>(k)};
+    CK(cudaMemcpyAsync(h.total.data(), d_tot, (size_t)k * 8, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
+    uint64_t run = 0; for (uint32_t i = 0; i < k; i++) { h.base[i] = run; run += align_up(h.total[i], 16); }
+    if (run >= (1ull << 32)) throw tfplan::FatalError(TF_E_FATAL_ARG, too_big);
+    heap.ensure(run + 256);
+    CK(cudaMemcpyAsync(d_base, h.base.data(), (size_t)k * 8, cudaMemcpyHostToDevice, s));
+    return h;
+}
+
+// A column descriptor over the buffers of `ic`, read as `type`; no output role yet.
+DCol make_dcol(const tf_col& ic, int type) {
+    DCol d; std::memset(&d, 0, sizeof d);
+    d.type = type; d.in_w = in_width(type); d.str_slot = -1; d.mask_slot = -1;
+    d.values = (const uint8_t*)ic.values; d.validity = ic.validity; d.offsets = ic.offsets; d.heap = ic.heap; d.aux = (const uint8_t*)ic.aux;
+    return d;
+}
+
+void ensure_d_cols(tfgpu_engine* e, size_t nc) {
+    if (e->d_cols_cap >= nc) return;
+    if (e->d_cols) CK(cudaFree(e->d_cols));
+    CK(cudaMalloc(&e->d_cols, sizeof(DCol) * nc)); e->d_cols_cap = nc;
+}
+
 // Launch the whole fused chain on e->stream. `cols_host` holds DEVICE pointers.
 #define TF_WIRE_COLUMNAR_INTERNAL 100
 // x-extent of a (tiles, slots) grid whose kernel strides over its tiles: enough CTAs for `waves` full waves of the device
@@ -330,29 +366,28 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
         throw tfplan::FatalError(TF_E_FATAL_UNSUPPORTED, "serializer sinks after convert_to_string on an `any` column are not handled on the device");
     const Sizes sz = compute_sizes(e, pd, in, columnar, json_rows);
     cudaStream_t s = e->stream;
-    // a pending checksum / gather tail may only stay in flight across a call that lays the work arena out identically
+    // a pending checksum kernel may only stay in flight across a call that lays the work arena out identically
     if (e->tail_pending && !(wire_fmt == TF_WIRE_CH_NATIVE_LZ4 && n == e->tail_nrows && (const void*)&pd == e->tail_plan && sz.n_frames_max == e->tail_nframes_max)) join_tail(e);
     // work arena
-    size_t wbytes = 0;
-    auto need = [&](size_t b) { wbytes += align_up(b ? b : 1, 256); };
-    need(n); need(n); need(n); need(sz.nblocks * 4); need(sz.nblocks * 4); need(n * 4);
     const size_t nslot_alloc = (size_t)(pd.n_str > 0 ? pd.n_str : 1);
-    need(nslot_alloc * sz.ntiles_cap * 4); need(nslot_alloc * sz.ntiles_cap * 8);
-    need(sz.n_frames_max * 4); need(sz.n_frames_max * 8); need(sz.n_frames_max * 8); need(256 * 8);
-    e->work.ensure(wbytes);
-    uint8_t* p = e->work.p;
-    e->keep = carve<uint8_t>(p, n); e->errcode = carve<uint8_t>(p, n); e->errstep = carve<uint8_t>(p, n);
-    e->blockcnt = carve<uint32_t>(p, sz.nblocks); e->blockoff = carve<uint32_t>(p, sz.nblocks); e->sel = carve<uint32_t>(p, n);
-    e->tile_sum = carve<uint32_t>(p, nslot_alloc * sz.ntiles_cap); e->tile_base = carve<uint64_t>(p, nslot_alloc * sz.ntiles_cap);
-    e->comp_size = carve<uint32_t>(p, sz.n_frames_max); e->wire_off = carve<uint64_t>(p, sz.n_frames_max); e->frame_pfx = carve<unsigned long long>(p, sz.n_frames_max); e->col_bytes = carve<uint64_t>(p, 256);
+    Layout W;
+    const size_t o_keep = W.take(n), o_errcode = W.take(n), o_errstep = W.take(n), o_blockcnt = W.take(sz.nblocks * 4), o_blockoff = W.take(sz.nblocks * 4),
+                 o_sel = W.take(n * 4), o_tile_sum = W.take(nslot_alloc * sz.ntiles_cap * 4), o_tile_base = W.take(nslot_alloc * sz.ntiles_cap * 8),
+                 o_comp = W.take(sz.n_frames_max * 4), o_wire_off = W.take(sz.n_frames_max * 8), o_pfx = W.take(sz.n_frames_max * 8), o_col_bytes = W.take(256 * 8);
+    e->work.ensure(W.total());
+    uint8_t* w = e->work.p;
+    e->keep = w + o_keep; e->errcode = w + o_errcode; e->errstep = w + o_errstep;
+    e->blockcnt = (uint32_t*)(w + o_blockcnt); e->blockoff = (uint32_t*)(w + o_blockoff); e->sel = (uint32_t*)(w + o_sel);
+    e->tile_sum = (uint32_t*)(w + o_tile_sum); e->tile_base = (uint64_t*)(w + o_tile_base);
+    e->comp_size = (uint32_t*)(w + o_comp); e->wire_off = (uint64_t*)(w + o_wire_off); e->frame_pfx = (unsigned long long*)(w + o_pfx); e->col_bytes = (uint64_t*)(w + o_col_bytes);
     e->raw.ensure(sz.raw_bound);
     const bool lz = wire_fmt == TF_WIRE_CH_NATIVE_LZ4;
     if (lz) e->wire.ensure(sz.wire_bound);
-    if (e->d_cols_cap < nc) { if (e->d_cols) CK(cudaFree(e->d_cols)); CK(cudaMalloc(&e->d_cols, sizeof(DCol) * nc)); e->d_cols_cap = nc; }
+    ensure_d_cols(e, nc);
     // column descriptors
     std::vector<DCol> hc(nc); std::vector<StrictCol> strict;
     for (size_t c = 0; c < nc; c++) {
-        const tf_col& ic = dev_cols[c]; DCol& d = hc[c]; std::memset(&d, 0, sizeof d);
+        const tf_col& ic = dev_cols[c];
         int ctype = ic.type;
         if (ic.type != pl.in_schema[c].tf) {        // a loose value type: Strictify it to the column's type first (strictify.go:46-157)
             const int st = ic.type, dt = pl.in_schema[c].tf;
@@ -361,11 +396,11 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
             else if (s_num && in_width(dt) && !(st == TF_FLOAT && dt == TF_DOUBLE) && !(st == TF_BOOLEAN && dt == TF_DOUBLE)) { strict.push_back(StrictCol{(const uint8_t*)ic.values, nullptr, ic.validity, st, dt, (int32_t)c, 0}); ctype = dt; }
             else throw tfplan::FatalError(TF_E_FATAL_ARG, "column " + std::to_string(c) + ": a " + std::to_string(st) + " value cannot be strictified to the plan's column type on the device");
         }
-        d.type = ctype; d.out_kind = pd.col_out_kind[c]; d.in_w = in_width(ctype); d.out_w = pd.col_out_w[c];
+        DCol& d = hc[c]; d = make_dcol(ic, ctype);
+        d.out_kind = pd.col_out_kind[c]; d.out_w = pd.col_out_w[c];
         if (columnar && d.out_kind == OK_TODT) d.out_w = 8;          // Transformed value is a time.Time: int64 seconds
         else if (columnar && d.out_kind != OK_STR && d.out_kind != OK_MASK && d.out_kind != OK_TOSTR) { d.out_kind = OK_COPY; d.out_w = d.in_w; }   // Transformed values keep their type
         d.nullable = pd.col_nullable[c]; d.str_slot = pd.col_str_slot[c]; d.mask_slot = pd.col_mask_slot[c];
-        d.values = (const uint8_t*)ic.values; d.validity = ic.validity; d.offsets = ic.offsets; d.heap = ic.heap; d.aux = (const uint8_t*)ic.aux;
         if (n) {
             if (d.in_w && !d.values) throw tfplan::FatalError(TF_E_FATAL_ARG, "column " + std::to_string(c) + ": values pointer is NULL");
             if (!d.in_w && !d.offsets) throw tfplan::FatalError(TF_E_FATAL_ARG, "column " + std::to_string(c) + ": offsets pointer is NULL");
@@ -374,11 +409,11 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
     if (!pre_err) e->prof_n = 0;
     const uint8_t* pre_term = nullptr;
     if (!strict.empty() && n) {        // Strictify pre-pass: loose fixed-width values -> the schema's type, range / cast failures as row errors
-        size_t sb = 0; auto need3 = [&](size_t b) { size_t at = sb; sb += align_up(b ? b : 1, 256); return at; };
-        const size_t o_desc = need3(strict.size() * sizeof(StrictCol)), o_err = need3(n), o_term = need3(n);
+        Layout S;
+        const size_t o_desc = S.take(strict.size() * sizeof(StrictCol)), o_err = S.take(n), o_term = S.take(n);
         std::vector<size_t> o_val(strict.size());
-        for (size_t k = 0; k < strict.size(); k++) o_val[k] = need3((size_t)in_width(strict[k].dst_tf) * n + 16);
-        e->strict_stage.ensure(sb + 256);
+        for (size_t k = 0; k < strict.size(); k++) o_val[k] = S.take((size_t)in_width(strict[k].dst_tf) * n + 16);
+        e->strict_stage.ensure(S.total() + 256);
         uint8_t* B = e->strict_stage.p;
         for (size_t k = 0; k < strict.size(); k++) { strict[k].dst = B + o_val[k]; hc[strict[k].col].values = B + o_val[k]; }
         CK(cudaMemcpyAsync(B + o_desc, strict.data(), strict.size() * sizeof(StrictCol), cudaMemcpyHostToDevice, s));
@@ -392,25 +427,20 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
     CK(cudaMemsetAsync(e->d_state, 0, sizeof(DState), s));
     if (!pl.n2f_cols.empty() && n) {        // number_to_float: rewrite the JSON text of the `any` columns before anything reads them
         const size_t k2 = pl.n2f_cols.size();
-        size_t sb = 0; auto need2 = [&](size_t b) { size_t at = sb; sb += align_up(b ? b : 1, 256); return at; };
-        const size_t o_which = need2(k2 * 4), o_len = need2(k2 * n * 4), o_off = need2(k2 * (n + 1) * 4), o_tot = need2(k2 * 8 + 8), o_base = need2(k2 * 8 + 8), o_err = need2(n);
-        e->n2f_stage.ensure(sb + 256);
+        Layout S;
+        const size_t o_which = S.take(k2 * 4), o_len = S.take(k2 * n * 4), o_off = S.take(k2 * (n + 1) * 4), o_tot = S.take(k2 * 8 + 8), o_base = S.take(k2 * 8 + 8), o_err = S.take(n);
+        e->n2f_stage.ensure(S.total() + 256);
         uint8_t* B = e->n2f_stage.p;
         std::vector<int32_t> which(pl.n2f_cols.begin(), pl.n2f_cols.end());
         CK(cudaMemcpyAsync(B + o_which, which.data(), k2 * 4, cudaMemcpyHostToDevice, s));
         if (pre_err) CK(cudaMemcpyAsync(B + o_err, pre_err, n, cudaMemcpyDeviceToDevice, s)); else CK(cudaMemsetAsync(B + o_err, 0, n, s));
         N2fArgs na{e->d_cols, (const int32_t*)(B + o_which), dev_kinds, n, (uint32_t*)(B + o_len), (const uint32_t*)(B + o_off), nullptr, (const uint64_t*)(B + o_base), B + o_err};
         e->prof_begin("k_n2f_sizes", s); launch_k_n2f_sizes(dim3((uint32_t)((n + 127) / 128), (uint32_t)k2), 128, 0, s, na); e->prof_end(s);
-        launch_offsets(e, (const uint32_t*)(B + o_len), n, (uint32_t)k2, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), s);
-        std::vector<uint64_t> tot(k2), base(k2);
-        CK(cudaMemcpyAsync(tot.data(), B + o_tot, k2 * 8, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
-        uint64_t run = 0; for (size_t k = 0; k < k2; k++) { base[k] = run; run += align_up(tot[k], 16); }
-        if (run >= (1ull << 32)) throw tfplan::FatalError(TF_E_FATAL_ARG, "number_to_float: a rewritten column exceeds 4 GiB");
-        e->n2f_heap.ensure(run + 256);
-        CK(cudaMemcpyAsync(B + o_base, base.data(), k2 * 8, cudaMemcpyHostToDevice, s));
+        const Heaps h = size_heaps(e, (const uint32_t*)(B + o_len), n, (uint32_t)k2, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), (uint64_t*)(B + o_base),
+                                   e->n2f_heap, "number_to_float: a rewritten column exceeds 4 GiB");
         na.heap = e->n2f_heap.p;
         e->prof_begin("k_n2f_write", s); launch_k_n2f_write(dim3((uint32_t)((n + 127) / 128), (uint32_t)k2), 128, 0, s, na); e->prof_end(s);
-        for (size_t k = 0; k < k2; k++) { DCol& d = hc[pl.n2f_cols[k]]; d.offsets = (const uint32_t*)(B + o_off) + k * (n + 1); d.heap = e->n2f_heap.p + base[k]; }
+        for (size_t k = 0; k < k2; k++) { DCol& d = hc[pl.n2f_cols[k]]; d.offsets = (const uint32_t*)(B + o_off) + k * (n + 1); d.heap = e->n2f_heap.p + h.base[k]; }
         CK(cudaMemcpyAsync(e->d_cols, hc.data(), sizeof(DCol) * nc, cudaMemcpyHostToDevice, s));
         pre_err = B + o_err;                 // parser errors carried over + N2F_HOST rows
     }
@@ -530,12 +560,12 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
         CK(cudaMemsetAsync(e->frame_pfx, 0, sz.n_frames_max * 8, s));
         // frames are compressed and written at their final wire offset by one kernel (sizes of the earlier frames by decoupled look-back)
         e->prof_begin("k_lz4_frames", s); launch_k_lz4_frames(grid, LZ_THREADS, smem, s, za); e->prof_end(s);
-        // the checksum chain (one thread per frame: latency-bound, a few warps per SM) runs on a side stream, under the next batch
+        // the checksum kernel (one thread per frame: latency-bound, a few warps per SM) runs on the side stream, under the next batch
         FrameArgs fa{e->comp_size, e->wire_off, e->wire.p, e->d_tail};
-        cudaStream_t s3 = e->side2_stream;
+        cudaStream_t s3 = e->side_stream;
         CK(cudaEventRecord(e->ev_fork, s)); CK(cudaStreamWaitEvent(s3, e->ev_fork, 0));
         e->prof_begin("k_frame_seal", s3); launch_k_frame_seal((uint32_t)((sz.n_frames_max + 31) / 32), 32, SEAL_SMEM, s3, fa); e->prof_end(s3);
-        CK(cudaEventRecord(e->ev_tail2, s3));
+        CK(cudaEventRecord(e->ev_tail, s3));
         e->tail_pending = true; e->tail_nrows = n; e->tail_plan = (const void*)&pd; e->tail_nframes_max = sz.n_frames_max;      // joined by whoever needs the wire bytes, or by the next batch before its LZ4
     }
     CK(cudaGetLastError());
@@ -574,10 +604,9 @@ int tfgpu_engine_create(const char* cfg_json, const int* device_ids, int n_devic
         CK(cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking));
         e->stream = e->own_stream;
         CK(cudaStreamCreateWithFlags(&e->side_stream, cudaStreamNonBlocking));
-        CK(cudaStreamCreateWithFlags(&e->side2_stream, cudaStreamNonBlocking));
-        CK(cudaEventCreateWithFlags(&e->ev_tail2, cudaEventDisableTiming));
+        CK(cudaEventCreateWithFlags(&e->ev_tail, cudaEventDisableTiming));
         CK(cudaMalloc(&e->d_tail, 64)); CK(cudaMemset(e->d_tail, 0, 64));
-        CK(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming)); CK(cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming));
+        CK(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
         CK(cudaMalloc(&e->d_state, sizeof(DState)));
         CK(lz4_kernels_init()); CK(dbz_kernels_init());
     } catch (const CudaError& c) { return c.e == cudaErrorMemoryAllocation ? TF_E_RETRY_OOM : TF_E_RETRY_LAUNCH; }
@@ -590,22 +619,18 @@ int tfgpu_engine_destroy(tfgpu_engine* e) {
     if (!e) return TF_E_FATAL_ARG;
     cudaSetDevice(e->device);
     cudaDeviceSynchronize();
-    for (auto& p : e->plans) p->consts.release();
-    e->strict_stage.release(); e->lens_arena.release(); e->lens_arena2.release(); e->in_arena.release(); e->work.release(); e->raw.release(); e->slots.release(); e->wire.release(); e->csv_text.release(); e->csv_stage.release(); e->json_msgs.release(); e->n2f_stage.release(); e->n2f_heap.release(); e->off_scratch.release(); e->json_sizes.release();
+    // the DevBufs (engine arenas, plan constants) free themselves in `delete e`
     if (e->d_state) cudaFree(e->d_state);
     if (e->d_cols) cudaFree(e->d_cols);
     if (e->d_call_slots) { cudaFree(e->d_call_slots); cudaFree(e->d_regions); }
+    if (e->d_tail) cudaFree(e->d_tail);
+    if (e->lz_phases) cudaFree(e->lz_phases);
     if (e->pinned) cudaFreeHost(e->pinned);
     if (e->sel_host) cudaFreeHost(e->sel_host);
     if (e->gather_pool) tfgpu_columnar_destroy(e->gather_pool);
-    e->sel_stage.release(); e->err_list.release();
     for (auto ev : e->prof_ev) cudaEventDestroy(ev);
     if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-    if (e->ev_join) cudaEventDestroy(e->ev_join);
-    if (e->ev_tail2) cudaEventDestroy(e->ev_tail2);
-    if (e->side2_stream) cudaStreamDestroy(e->side2_stream);
-    if (e->d_tail) cudaFree(e->d_tail);
-    e->dbz_keysz.release(); e->dbz_meta.release(); e->dbz_old.release(); e->dbz_msgsz.release(); e->old_arena.release(); e->part_ids.release();
+    if (e->ev_tail) cudaEventDestroy(e->ev_tail);
     if (e->side_stream) cudaStreamDestroy(e->side_stream);
     if (e->own_stream) cudaStreamDestroy(e->own_stream);
     delete e;
@@ -619,8 +644,7 @@ int tfgpu_profile_enable(tfgpu_engine* e, int on) { if (!e) return TF_E_FATAL_AR
 
 const char* tfgpu_profile_read(tfgpu_engine* e) {
     if (!e) return nullptr;
-    cudaSetDevice(e->device);
-    try { join_tail(e); } catch (const CudaError&) {}
+    on_device(e, [&] { join_tail(e); return TF_OK; });
     cudaStreamSynchronize(e->stream);
     std::string j = "[";
     for (int i = 0; i < e->prof_n; i++) {
@@ -633,7 +657,7 @@ const char* tfgpu_profile_read(tfgpu_engine* e) {
 
 int tfgpu_engine_set_stream(tfgpu_engine* e, void* cuda_stream) {
     if (!e) return TF_E_FATAL_ARG;
-    if (e->tail_pending) { cudaSetDevice(e->device); cudaStreamSynchronize(e->side_stream); cudaStreamSynchronize(e->side2_stream); e->tail_pending = false; }
+    if (e->tail_pending) { cudaSetDevice(e->device); cudaStreamSynchronize(e->side_stream); e->tail_pending = false; }
     e->stream = cuda_stream ? (cudaStream_t)cuda_stream : e->own_stream;
     return TF_OK;
 }
@@ -641,33 +665,14 @@ int tfgpu_engine_set_stream(tfgpu_engine* e, void* cuda_stream) {
 int tfgpu_plan(tfgpu_engine* e, const char* ns, const char* name, const char* schema_json, const char* transformers_json,
                const char* sink_json, int* plan_id) {
     if (!e || !schema_json || !plan_id || !name) return TF_E_FATAL_ARG;
-    try {
-        CK(cudaSetDevice(e->device));
+    return on_device(e, [&] {
         auto pd = std::make_unique<PlanDev>();
         pd->plan = tfplan::build_plan(ns ? ns : "", name, schema_json, transformers_json ? transformers_json : "", sink_json ? sink_json : "");
-        upload_plan(e, *pd);
+        upload_plan(*pd);
         e->plans.push_back(std::move(pd));
         *plan_id = (int)e->plans.size() - 1;
         return TF_OK;
-    } catch (const tfplan::FatalError& f) { return fail(e, f.code, f.what()); }
-    catch (const CudaError& c) { return cuda_fail(e, c); }
-    catch (const std::exception& x) { return fail(e, TF_E_FATAL_CONFIG, x.what()); }
-}
-
-// Host-only: build the plan (Suitable / ResultSchema chain, filter grammar, ClickHouse types) without touching a
-// device, so a transfer's YAML can be validated where no GPU is present (cmd/trcli validate does the same for the
-// reference's transformers: cmd/trcli/config/model.go:57-72).
-int tfgpu_plan_validate(const char* ns, const char* name, const char* schema_json, const char* transformers_json,
-                        const char* sink_json, char* describe_out, uint64_t cap, char* err_out, uint64_t err_cap) {
-    auto put = [](char* dst, uint64_t cap_, const std::string& s) { if (dst && cap_) { size_t n = s.size() < cap_ - 1 ? s.size() : cap_ - 1; std::memcpy(dst, s.data(), n); dst[n] = 0; } };
-    if (!schema_json || !name) return TF_E_FATAL_ARG;
-    try {
-        tfplan::Plan pl = tfplan::build_plan(ns ? ns : "", name, schema_json, transformers_json ? transformers_json : "", sink_json ? sink_json : "");
-        if (describe_out && pl.describe.size() + 1 > cap) { put(err_out, err_cap, "describe buffer too small"); return TF_E_FATAL_ARG; }
-        put(describe_out, cap, pl.describe);
-        return TF_OK;
-    } catch (const tfplan::FatalError& f) { put(err_out, err_cap, f.what()); return f.code; }
-    catch (const std::exception& x) { put(err_out, err_cap, x.what()); return TF_E_FATAL_CONFIG; }
+    });
 }
 
 const char* tfgpu_plan_describe(tfgpu_engine* e, int plan_id) {
@@ -684,32 +689,28 @@ int tfgpu_push_encode_resident(tfgpu_engine* e, int plan_id, int wire_fmt, const
     if (in->ncols != pd.plan.in_schema.size()) return fail(e, TF_E_FATAL_ARG, "batch column count does not match the plan schema");
     if (wire_fmt != TF_WIRE_CH_NATIVE && wire_fmt != TF_WIRE_CH_NATIVE_LZ4) return fail(e, TF_E_FATAL_UNSUPPORTED, "wire format not implemented");
     if (in->nrows >= (1ull << 31)) return fail(e, TF_E_FATAL_ARG, "batch too large (>= 2^31 rows)");
-    try {
-        CK(cudaSetDevice(e->device));
+    return on_device(e, [&] {
         std::vector<tf_col> dev; const uint8_t* dev_kinds = stage_input(e, in, dev);    // device pointers pass through; TF_COL_LENS8 / 16 lengths become offsets
         run_chain(e, pd, in, dev.data(), dev_kinds, wire_fmt);
         return TF_OK;
-    } catch (const tfplan::FatalError& f) { return fail(e, f.code, f.what()); }
-    catch (const CudaError& c) { return cuda_fail(e, c); }
+    });
 }
 
 int tfgpu_resident_stats(tfgpu_engine* e, uint64_t* rows_out, uint64_t* raw_bytes, uint64_t* wire_bytes, uint64_t* n_errors) {
     if (!e) return TF_E_FATAL_ARG;
-    try {
-        CK(cudaSetDevice(e->device));
+    return on_device(e, [&] {
         join_tail(e);
         DState st; CK(cudaMemcpyAsync(&st, e->d_state, sizeof st, cudaMemcpyDeviceToHost, e->stream)); CK(cudaStreamSynchronize(e->stream));
         if (rows_out) *rows_out = st.n_kept; if (raw_bytes) *raw_bytes = st.raw_total;
         if (wire_bytes) *wire_bytes = e->last_wire_fmt == TF_WIRE_CH_NATIVE_LZ4 ? st.wire_total : st.raw_total;
         if (n_errors) *n_errors = st.n_errors;
         return TF_OK;
-    } catch (const CudaError& c) { return cuda_fail(e, c); }
+    });
 }
 
 int tfgpu_resident_fetch(tfgpu_engine* e, int what, uint8_t* dst, uint64_t cap) {
     if (!e || !dst) return TF_E_FATAL_ARG;
-    try {
-        CK(cudaSetDevice(e->device));
+    return on_device(e, [&] {
         join_tail(e);
         DState st; CK(cudaMemcpyAsync(&st, e->d_state, sizeof st, cudaMemcpyDeviceToHost, e->stream)); CK(cudaStreamSynchronize(e->stream));
         const bool wire = what == 1 && e->last_wire_fmt == TF_WIRE_CH_NATIVE_LZ4;
@@ -717,7 +718,7 @@ int tfgpu_resident_fetch(tfgpu_engine* e, int what, uint8_t* dst, uint64_t cap) 
         if (n > cap) return fail(e, TF_E_FATAL_ARG, "destination too small");
         CK(cudaMemcpyAsync(dst, wire ? e->wire.p : e->raw.p, n, cudaMemcpyDeviceToHost, e->stream)); CK(cudaStreamSynchronize(e->stream));
         return TF_OK;
-    } catch (const CudaError& c) { return cuda_fail(e, c); }
+    });
 }
 
 static void fetch_errors(tfgpu_engine* e, uint64_t n, tfgpu_result* r);
@@ -731,19 +732,14 @@ int tfgpu_push_encode(tfgpu_engine* e, int plan_id, int wire_fmt, const tf_batch
     if (!wire_is_ser(wire_fmt) && !pd.plan.has_sink) return fail(e, TF_E_FATAL_CONFIG, "plan was built without a sink");
     if (in->ncols != pd.plan.in_schema.size()) return fail(e, TF_E_FATAL_ARG, "batch column count does not match the plan schema");
     if (in->nrows >= (1ull << 31)) return fail(e, TF_E_FATAL_ARG, "batch too large (>= 2^31 rows)");
-    try {
-        CK(cudaSetDevice(e->device));
-        const uint64_t n = in->nrows;
+    return on_device(e, [&] {
         std::vector<tf_col> dev; const uint8_t* dev_kinds = stage_input(e, in, dev);
-        cudaStream_t s = e->stream;
         run_chain(e, pd, in, dev.data(), dev_kinds, wire_fmt);
         auto r = std::make_unique<tfgpu_result>();
-        finish_wire(e, n, wire_fmt, r.get());
+        finish_wire(e, in->nrows, wire_fmt, r.get());
         *out = r.release();
         return TF_OK;
-    } catch (const tfplan::FatalError& f) { return fail(e, f.code, f.what()); }
-    catch (const CudaError& c) { return cuda_fail(e, c); }
-    catch (const std::bad_alloc&) { return fail(e, TF_E_RETRY_OOM, "host allocation failed"); }
+    });
 }
 
 // Two-phase push: only the predicate columns cross PCIe first; k_filter answers with the keep flags; the host gathers the kept rows
@@ -759,8 +755,7 @@ int tfgpu_push_encode_selective(tfgpu_engine* e, int plan_id, int wire_fmt, cons
     for (const auto& fs : pl.filters) for (const auto& ex : fs.exprs) for (const auto& t : ex) if (t.col >= 0 && (size_t)t.col < nc) pred[t.col] = 1;
     for (size_t c = 0; c < nc; c++) if (pred[c] && in->cols[c].type != pl.in_schema[c].tf) return tfgpu_push_encode(e, plan_id, wire_fmt, in, out);   // loose predicate column: Strictify first, one phase
     *out = nullptr;
-    try {
-        CK(cudaSetDevice(e->device));
+    return on_device(e, [&] {
         join_tail(e);
         cudaStream_t s = e->stream;
         static const bool trace = std::getenv("TFGPU_SELECTIVE_TRACE") != nullptr;
@@ -771,19 +766,16 @@ int tfgpu_push_encode_selective(tfgpu_engine* e, int plan_id, int wire_fmt, cons
         const tf_batch b1{n, (uint32_t)nc, TF_MEM_HOST, pc.data(), in->kinds};
         std::vector<tf_col> dev; const uint8_t* dev_kinds = stage_input(e, &b1, dev);
         std::vector<DCol> hc(nc);
-        for (size_t c = 0; c < nc; c++) {
-            DCol& d = hc[c]; std::memset(&d, 0, sizeof d);
-            d.type = pl.in_schema[c].tf; d.in_w = in_width(d.type); d.str_slot = -1; d.mask_slot = -1;
-            d.values = (const uint8_t*)dev[c].values; d.validity = dev[c].validity; d.offsets = dev[c].offsets; d.heap = dev[c].heap; d.aux = (const uint8_t*)dev[c].aux;
-        }
-        if (e->d_cols_cap < nc) { if (e->d_cols) CK(cudaFree(e->d_cols)); CK(cudaMalloc(&e->d_cols, sizeof(DCol) * nc)); e->d_cols_cap = nc; }
+        for (size_t c = 0; c < nc; c++) hc[c] = make_dcol(dev[c], pl.in_schema[c].tf);
+        ensure_d_cols(e, nc);
         CK(cudaMemcpyAsync(e->d_cols, hc.data(), sizeof(DCol) * nc, cudaMemcpyHostToDevice, s));
         CK(cudaMemsetAsync(e->d_state, 0, sizeof(DState), s));
         const uint32_t nb = (uint32_t)((n + 255) / 256);
-        const size_t flags_bytes = align_up(3 * n, 256);
-        e->sel_stage.ensure(flags_bytes + (size_t)nb * 4 + 256);
-        uint8_t* B = e->sel_stage.p;
-        FilterArgs fa{e->d_cols, dev_kinds, n, pd.d_fsteps, pd.n_fsteps, pd.d_expr_off, pd.d_terms, pd.d_blob, B, B + n, B + 2 * n, (uint32_t*)(B + flags_bytes), e->d_state, nullptr, nullptr, 0};
+        Layout L;
+        const size_t o_flags = L.take(3 * n), o_blockcnt = L.take((size_t)nb * 4);     // keep, errcode, errstep back to back: one copy to the host
+        e->sel_stage.ensure(L.total() + 256);
+        uint8_t* B = e->sel_stage.p + o_flags;
+        FilterArgs fa{e->d_cols, dev_kinds, n, pd.d_fsteps, pd.n_fsteps, pd.d_expr_off, pd.d_terms, pd.d_blob, B, B + n, B + 2 * n, (uint32_t*)(e->sel_stage.p + o_blockcnt), e->d_state, nullptr, nullptr, 0};
         e->prof_n = 0;
         e->prof_begin("k_filter", s); launch_k_filter(nb, 256, 0, s, fa); e->prof_end(s);
         if (e->sel_host_cap < 3 * n) { if (e->sel_host) CK(cudaFreeHost(e->sel_host)); e->sel_host = nullptr; e->sel_host_cap = 0; const size_t want = align_up(3 * n + 3 * n / 4 + 4096, 1 << 16); CK(cudaMallocHost(&e->sel_host, want)); e->sel_host_cap = want; }
@@ -818,91 +810,75 @@ int tfgpu_push_encode_selective(tfgpu_engine* e, int plan_id, int wire_fmt, cons
         }
         *out = r.release();
         return TF_OK;
-    } catch (const tfplan::FatalError& f) { return fail(e, f.code, f.what()); }
-    catch (const CudaError& c) { return cuda_fail(e, c); }
-    catch (const std::bad_alloc&) { return fail(e, TF_E_RETRY_OOM, "host allocation failed"); }
+    });
 }
 uint64_t tfgpu_engine_h2d_bytes(const tfgpu_engine* e) { return e ? e->h2d_bytes : 0; }
+
+// var-width columns that carry lengths instead of offsets (TF_COL_LENS8 / 16): offsets are built on the device, in `larena`
+static void expand_lens(tfgpu_engine* e, uint64_t nr, std::vector<tf_col>& dv, DevBuf& larena) {
+    std::vector<LensSrc> src; std::vector<uint32_t> which;
+    for (uint32_t c = 0; c < dv.size(); c++) if (!in_width(dv[c].type) && (dv[c].flags & (TF_COL_LENS8 | TF_COL_LENS16)) && dv[c].offsets) { src.push_back(LensSrc{(const uint8_t*)dv[c].offsets, (dv[c].flags & TF_COL_LENS8) ? 1 : 2, 0}); which.push_back(c); }
+    if (src.empty()) return;
+    const size_t K = src.size();
+    Layout L(16);
+    const size_t o_src = L.take(K * sizeof(LensSrc)), o_len = L.take(K * nr * 4), o_off = L.take(K * (nr + 1) * 4), o_tot = L.take(K * 8);
+    larena.ensure(L.total() + 256);
+    uint8_t* B = larena.p; cudaStream_t st = e->stream;
+    CK(cudaMemcpyAsync(B + o_src, src.data(), K * sizeof(LensSrc), cudaMemcpyHostToDevice, st));
+    // `src` is pageable: cudaMemcpyAsync has staged it before it returns, so the vector may go out of scope and nothing waits here
+    if (nr) { e->launches++; launch_k_widen_lens(dim3((uint32_t)std::min<uint64_t>((nr + 255) / 256, 2048), (uint32_t)K), 256, 0, st, (const LensSrc*)(B + o_src), nr, (uint32_t*)(B + o_len)); }
+    launch_offsets(e, (const uint32_t*)(B + o_len), nr, (uint32_t)K, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), st);
+    for (size_t k = 0; k < K; k++) { dv[which[k]].offsets = (const uint32_t*)(B + o_off) + k * (nr + 1); dv[which[k]].flags &= ~(TF_COL_LENS8 | TF_COL_LENS16); }
+}
 
 // shared by push_encode / push_columns: stage host columns into HBM (or pass device pointers through)
 static const uint8_t* stage_input(tfgpu_engine* e, const tf_batch* in, std::vector<tf_col>& dev, DevBuf* arena_opt) {
     DevBuf& arena = arena_opt ? *arena_opt : e->in_arena;
     DevBuf& larena = arena_opt ? e->lens_arena2 : e->lens_arena;
-    // var-width columns that carry lengths instead of offsets (TF_COL_LENS8 / 16): offsets are built on the device
-    auto expand_lens = [&](std::vector<tf_col>& dv) {
-        const uint64_t nr = in->nrows; std::vector<LensSrc> src; std::vector<uint32_t> which;
-        for (uint32_t c = 0; c < in->ncols; c++) if (!in_width(dv[c].type) && (dv[c].flags & (TF_COL_LENS8 | TF_COL_LENS16)) && dv[c].offsets) { src.push_back(LensSrc{(const uint8_t*)dv[c].offsets, (dv[c].flags & TF_COL_LENS8) ? 1 : 2, 0}); which.push_back(c); }
-        if (src.empty()) return;
-        const size_t K = src.size(), o_src = 0, o_len = align_up(K * sizeof(LensSrc) + 16, 256), o_off = o_len + align_up(K * nr * 4 + 16, 256), o_tot = o_off + align_up(K * (nr + 1) * 4 + 16, 256);
-        larena.ensure(o_tot + K * 8 + 256);
-        uint8_t* B = larena.p; cudaStream_t st = e->stream;
-        CK(cudaMemcpyAsync(B + o_src, src.data(), K * sizeof(LensSrc), cudaMemcpyHostToDevice, st));
-        // `src` is pageable: cudaMemcpyAsync has staged it before it returns, so the vector may go out of scope and nothing waits here
-        if (nr) { e->launches++; launch_k_widen_lens(dim3((uint32_t)std::min<uint64_t>((nr + 255) / 256, 2048), (uint32_t)K), 256, 0, st, (const LensSrc*)(B + o_src), nr, (uint32_t*)(B + o_len)); }
-        launch_offsets(e, (const uint32_t*)(B + o_len), nr, (uint32_t)K, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), st);
-        for (size_t k = 0; k < K; k++) { dv[which[k]].offsets = (const uint32_t*)(B + o_off) + k * (nr + 1); dv[which[k]].flags &= ~(TF_COL_LENS8 | TF_COL_LENS16); }
-    };
     const uint64_t n = in->nrows; const uint32_t nc = in->ncols;
     cudaStream_t s = e->stream;
     dev.resize(nc);
-    if (in->mem != TF_MEM_HOST) { for (uint32_t c = 0; c < nc; c++) dev[c] = in->cols[c]; expand_lens(dev); return in->kinds; }
-    size_t tot = 0;
-    auto sz_of = [&](const tf_col& c, int which) -> size_t {
-        const int w = in_width(c.type);
-        switch (which) {
-        case 0: return w ? (size_t)w * n : 0;
-        case 1: return c.validity ? (n + 7) / 8 : 0;
-        case 2: return (!w && c.offsets) ? ((c.flags & TF_COL_LENS8) ? n : (c.flags & TF_COL_LENS16) ? 2 * n : (n + 1) * 4) : 0;
-        case 3: return (!w) ? c.heap_len : 0;
-        default: if (!c.aux) return 0; return (c.type == TF_ANY) ? n : (size_t)4 * n;
-        }
-    };
-    for (uint32_t c = 0; c < nc; c++) for (int k = 0; k < 5; k++) tot += align_up(sz_of(in->cols[c], k) + 16, 256);
-    tot += align_up(n + 16, 256);
-    arena.ensure(tot);
-    uint8_t* p = arena.p;
-    // A shim that keeps the whole batch in ONE pinned arena laid out like the device staging (every non-empty buffer at the next multiple of
-    // 256 past the previous buffer's end + 16, in the order values / validity / offsets / heap / aux per column, then kinds) gets a single
-    // DMA instead of one per buffer: a few hundred descriptors per batch cost several per cent of the PCIe time.
-    {
-        const uint8_t* first = nullptr; size_t first_off = 0, off = 0, end_off = 0; bool contiguous = true;
-        auto chk = [&](const void* src, size_t bytes) {
-            if (!src || !bytes) return;
-            if (!first) { first = (const uint8_t*)src; first_off = off; }
-            else if ((const uint8_t*)src != first + (off - first_off)) contiguous = false;
-            end_off = off + bytes; off += align_up(bytes + 16, 256);
-        };
-        for (uint32_t c = 0; c < nc && contiguous; c++) { const tf_col& ic = in->cols[c]; chk(ic.values, sz_of(ic, 0)); chk(ic.validity, sz_of(ic, 1)); chk(ic.offsets, sz_of(ic, 2)); chk(ic.heap, sz_of(ic, 3)); chk(ic.aux, sz_of(ic, 4)); }
-        if (contiguous && in->kinds) chk(in->kinds, n);
-        if (contiguous && first && end_off - first_off >= (1u << 20)) {
-            CK(cudaMemcpyAsync(p + first_off, first, end_off - first_off, cudaMemcpyHostToDevice, s)); e->h2d_bytes += end_off - first_off;
-            auto at = [&](const void* src, size_t bytes) -> uint8_t* { if (!src || !bytes) return nullptr; uint8_t* d = p; p += align_up(bytes + 16, 256); return d; };
-            for (uint32_t c = 0; c < nc; c++) {
-                const tf_col& ic = in->cols[c]; tf_col& d = dev[c]; d = ic;
-                d.values = at(ic.values, sz_of(ic, 0)); d.validity = at(ic.validity, sz_of(ic, 1)); d.offsets = (const uint32_t*)at(ic.offsets, sz_of(ic, 2));
-                d.heap = at(ic.heap, sz_of(ic, 3)); if (!in_width(ic.type) && !d.heap) d.heap = arena.p;
-                d.aux = at(ic.aux, sz_of(ic, 4));
-            }
-            const uint8_t* dk1 = in->kinds ? at(in->kinds, n) : nullptr;
-            expand_lens(dev);
-            return dk1;
-        }
-    }
-    auto up = [&](const void* src, size_t bytes) -> uint8_t* {
-        if (!src || !bytes) { return nullptr; }
-        uint8_t* d = p; CK(cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, s)); p += align_up(bytes + 16, 256); e->h2d_bytes += bytes; return d;
-    };
+    if (in->mem != TF_MEM_HOST) { for (uint32_t c = 0; c < nc; c++) dev[c] = in->cols[c]; expand_lens(e, n, dev, larena); return in->kinds; }
+    // every non-empty buffer in the order values / validity / offsets / heap / aux per column, then kinds
+    const size_t nb = 5 * (size_t)nc + 1;
+    std::vector<const uint8_t*> src(nb); std::vector<size_t> bytes(nb);
     for (uint32_t c = 0; c < nc; c++) {
-        const tf_col& ic = in->cols[c]; tf_col& d = dev[c]; d = ic;
-        d.values = up(ic.values, sz_of(ic, 0)); d.validity = up(ic.validity, sz_of(ic, 1));
-        d.offsets = (const uint32_t*)up(ic.offsets, sz_of(ic, 2));
-        d.heap = up(ic.heap, sz_of(ic, 3));
-        if (!in_width(ic.type) && !d.heap) d.heap = arena.p;   // empty heap: any valid pointer
-        d.aux = up(ic.aux, sz_of(ic, 4));
+        const tf_col& ic = in->cols[c]; const int w = in_width(ic.type); const size_t k = 5 * (size_t)c;
+        src[k] = (const uint8_t*)ic.values;   bytes[k] = w ? (size_t)w * n : 0;
+        src[k + 1] = ic.validity;             bytes[k + 1] = ic.validity ? (n + 7) / 8 : 0;
+        src[k + 2] = (const uint8_t*)ic.offsets; bytes[k + 2] = (!w && ic.offsets) ? ((ic.flags & TF_COL_LENS8) ? n : (ic.flags & TF_COL_LENS16) ? 2 * n : (n + 1) * 4) : 0;
+        src[k + 3] = ic.heap;                 bytes[k + 3] = !w ? ic.heap_len : 0;
+        src[k + 4] = (const uint8_t*)ic.aux;  bytes[k + 4] = ic.aux ? ((ic.type == TF_ANY) ? n : (size_t)4 * n) : 0;
     }
-    const uint8_t* dk = in->kinds ? up(in->kinds, n) : nullptr;
-    expand_lens(dev);
-    return dk;
+    src[nb - 1] = in->kinds; bytes[nb - 1] = in->kinds ? n : 0;
+    // A shim that keeps the whole batch in ONE pinned arena laid out like the device staging (abi.Batch.pin_arena) gets a single DMA instead
+    // of one per buffer: a few hundred descriptors per batch cost several per cent of the PCIe time.
+    Layout L(16); std::vector<size_t> at(nb);
+    const uint8_t* first = nullptr; size_t first_at = 0, end_at = 0; bool contiguous = true;
+    for (size_t i = 0; i < nb; i++) {
+        if (!src[i] || !bytes[i]) continue;
+        at[i] = L.take(bytes[i]);
+        if (!first) { first = src[i]; first_at = at[i]; }
+        else if (src[i] != first + (at[i] - first_at)) contiguous = false;
+        end_at = at[i] + bytes[i];
+    }
+    arena.ensure(L.total() + 256);
+    uint8_t* B = arena.p;
+    const bool one_dma = contiguous && first && end_at - first_at >= (1u << 20);
+    if (one_dma) { CK(cudaMemcpyAsync(B + first_at, first, end_at - first_at, cudaMemcpyHostToDevice, s)); e->h2d_bytes += end_at - first_at; }
+    std::vector<uint8_t*> d(nb, nullptr);
+    for (size_t i = 0; i < nb; i++) {
+        if (!src[i] || !bytes[i]) continue;
+        d[i] = B + at[i];
+        if (!one_dma) { CK(cudaMemcpyAsync(d[i], src[i], bytes[i], cudaMemcpyHostToDevice, s)); e->h2d_bytes += bytes[i]; }
+    }
+    for (uint32_t c = 0; c < nc; c++) {
+        const size_t k = 5 * (size_t)c; tf_col& dc = dev[c]; dc = in->cols[c];
+        dc.values = d[k]; dc.validity = d[k + 1]; dc.offsets = (const uint32_t*)d[k + 2]; dc.heap = d[k + 3]; dc.aux = d[k + 4];
+        if (!in_width(dc.type) && !dc.heap) dc.heap = B;   // empty heap: any valid pointer
+    }
+    expand_lens(e, n, dev, larena);
+    return d[nb - 1];
 }
 
 static void fetch_errors(tfgpu_engine* e, uint64_t n, tfgpu_result* r) {
@@ -987,31 +963,24 @@ int tfgpu_push_columns(tfgpu_engine* e, int plan_id, const tf_batch* in, tfgpu_r
     PlanDev& pd = *e->plans[plan_id];
     if (in->ncols != pd.plan.in_schema.size()) return fail(e, TF_E_FATAL_ARG, "batch column count does not match the plan schema");
     if (in->nrows >= (1ull << 31)) return fail(e, TF_E_FATAL_ARG, "batch too large (>= 2^31 rows)");
-    try {
-        CK(cudaSetDevice(e->device));
+    return on_device(e, [&] {
         std::vector<tf_col> dev; const uint8_t* dev_kinds = stage_input(e, in, dev);
         run_chain(e, pd, in, dev.data(), dev_kinds, TF_WIRE_COLUMNAR_INTERNAL);
         auto r = std::make_unique<tfgpu_result>();
         finish_columnar(e, pd, in->nrows, r.get());
         *out = r.release();
         return TF_OK;
-    } catch (const tfplan::FatalError& f) { return fail(e, f.code, f.what()); }
-    catch (const CudaError& c) { return cuda_fail(e, c); }
-    catch (const std::bad_alloc&) { return fail(e, TF_E_RETRY_OOM, "host allocation failed"); }
+    });
 }
 
 // Queue Debezium serializer for columns without a database-specific original_type (Emitter.EmitKV
 // pkg/debezium/emitter_value_converter.go:626-690). The per-table constants become a text template once per (plan, opts).
 namespace {
-__global__ void k_dbz_kinds(const uint8_t* kinds, uint64_t n, uint8_t* pre_err) {
-    const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r < n) pre_err[r] = kinds[r] == TF_KIND_INSERT ? 0 : TF_ROWERR_DBZ_EMIT_HOST;
-}
 // Host part of the emitter set-up, independent of any device state (tfgpu_emit_debezium_validate exports it for tests without a GPU):
 // the AddPg / addCommon branch of every result column and the message template.
 struct DbzHostTpl { std::vector<int> forms; std::string text; std::vector<DbzSeg> segs; };
-DbzHostTpl dbz_host_template(const tfplan::Plan& pl, const std::string& opts_json) {
-    auto ov = tfj::parse(opts_json);
+DbzHostTpl dbz_host_template(const tfplan::Plan& pl, const tfj::Value& opts) {
+    const tfj::Value* ov = &opts;
 
     // per result column: addCommon, or the AddPg branch (pkg/debezium/pg/emitter.go:265-629) its (original type, column type) pair takes
     std::vector<int> forms(pl.out_schema.size(), DF_COMMON); bool any_common = false;
@@ -1086,22 +1055,20 @@ DbzHostTpl dbz_host_template(const tfplan::Plan& pl, const std::string& opts_jso
     return t;
 }
 
-void dbz_build_template(PlanDev& pd, const std::string& opts_json) {
+void dbz_build_template(PlanDev& pd, const std::string& opts_json, const tfj::Value& opts) {
     if (pd.dbz_opts_key == opts_json && pd.dbz.segs) return;
     const tfplan::Plan& pl = pd.plan;
-    const DbzHostTpl ht = dbz_host_template(pl, opts_json);
+    const DbzHostTpl ht = dbz_host_template(pl, opts);
     const std::vector<int>& forms = ht.forms; const std::string& text = ht.text; const std::vector<DbzSeg>& segs = ht.segs;
     std::vector<JsonCol> acols = pd.h_sjcols, kcols;
     for (JsonCol& jc : acols) jc.pad1 = forms[(size_t)jc.pad0];
     for (const JsonCol& jc : acols) if (pl.out_schema[(size_t)jc.pad0].key) kcols.push_back(jc);
-    const size_t o_seg = 0, o_text = align_up(segs.size() * sizeof(DbzSeg), 256), o_k = o_text + align_up(text.size() + 1, 256), o_a = o_k + align_up(kcols.size() * sizeof(JsonCol) + 1, 256);
-    pd.dbz_consts.ensure(o_a + acols.size() * sizeof(JsonCol) + 256);
-    if (!acols.empty()) CK(cudaMemcpy(pd.dbz_consts.p + o_a, acols.data(), acols.size() * sizeof(JsonCol), cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(pd.dbz_consts.p + o_seg, segs.data(), segs.size() * sizeof(DbzSeg), cudaMemcpyHostToDevice));
-    if (!text.empty()) CK(cudaMemcpy(pd.dbz_consts.p + o_text, text.data(), text.size(), cudaMemcpyHostToDevice));
-    if (!kcols.empty()) CK(cudaMemcpy(pd.dbz_consts.p + o_k, kcols.data(), kcols.size() * sizeof(JsonCol), cudaMemcpyHostToDevice));
-    pd.dbz = DbzEmitArgs{}; pd.dbz.segs = (const DbzSeg*)(pd.dbz_consts.p + o_seg); pd.dbz.nseg = (int)segs.size(); pd.dbz.text = pd.dbz_consts.p + o_text;
-    pd.dbz.kcols = (const JsonCol*)(pd.dbz_consts.p + o_k); pd.dbz.nkc = (int)kcols.size(); pd.dbz.acols = (const JsonCol*)(pd.dbz_consts.p + o_a);
+    ConstImage ci;
+    const size_t o_seg = ci.add(segs.data(), segs.size() * sizeof(DbzSeg)), o_text = ci.add(text.c_str(), text.size() + 1),
+                 o_k = ci.add(kcols.data(), kcols.size() * sizeof(JsonCol)), o_a = ci.add(acols.data(), acols.size() * sizeof(JsonCol));
+    uint8_t* P = ci.upload(pd.dbz_consts);
+    pd.dbz = DbzEmitArgs{}; pd.dbz.segs = (const DbzSeg*)(P + o_seg); pd.dbz.nseg = (int)segs.size(); pd.dbz.text = P + o_text;
+    pd.dbz.kcols = (const JsonCol*)(P + o_k); pd.dbz.nkc = (int)kcols.size(); pd.dbz.acols = (const JsonCol*)(P + o_a);
     pd.dbz_opts_key = opts_json;
 }
 }  // namespace
@@ -1110,11 +1077,10 @@ void dbz_build_template(PlanDev& pd, const std::string& opts_json) {
 // {"forms":[per result column],"keys":[result column indexes in key-message order],"template":[[text, code], ...]}.
 int tfgpu_emit_debezium_validate(const char* ns, const char* name, const char* schema_json, const char* transformers_json, const char* opts_json,
                                  char* describe_out, uint64_t cap, char* err_out, uint64_t err_cap) {
-    auto put = [](char* dst, uint64_t cap_, const std::string& s) { if (dst && cap_) { size_t n = s.size() < cap_ - 1 ? s.size() : cap_ - 1; std::memcpy(dst, s.data(), n); dst[n] = 0; } };
     if (!schema_json || !name || !opts_json) return TF_E_FATAL_ARG;
-    try {
+    return host_validate(describe_out, cap, err_out, err_cap, [&] {
         const tfplan::Plan pl = tfplan::build_plan(ns ? ns : "", name, schema_json, transformers_json ? transformers_json : "", "");
-        const DbzHostTpl t = dbz_host_template(pl, opts_json);
+        const DbzHostTpl t = dbz_host_template(pl, *tfj::parse(opts_json));
         std::vector<size_t> order(pl.out_schema.size()); for (size_t k = 0; k < order.size(); k++) order[k] = k;
         std::stable_sort(order.begin(), order.end(), [&](size_t a, size_t b) { return pl.out_schema[a].name < pl.out_schema[b].name; });
         std::string d = "{\"forms\":[";
@@ -1127,11 +1093,8 @@ int tfgpu_emit_debezium_validate(const char* ns, const char* name, const char* s
             d += "[" + host_json_quote_nohtml(t.text.substr((size_t)t.segs[g].text_off, (size_t)t.segs[g].text_len)) + "," + std::to_string(t.segs[g].code) + "]";
         }
         d += "]}";
-        if (describe_out && d.size() + 1 > cap) { put(err_out, err_cap, "describe buffer too small"); return TF_E_FATAL_ARG; }
-        put(describe_out, cap, d);
-        return TF_OK;
-    } catch (const tfplan::FatalError& f) { put(err_out, err_cap, f.what()); return f.code; }
-    catch (const std::exception& x) { put(err_out, err_cap, x.what()); return TF_E_FATAL_CONFIG; }
+        return d;
+    });
 }
 
 int tfgpu_emit_debezium(tfgpu_engine* e, int plan_id, const char* opts_json, const tf_batch* in, const tf_row_meta* meta, tfgpu_result** out) {
@@ -1144,17 +1107,18 @@ int tfgpu_emit_debezium_crud(tfgpu_engine* e, int plan_id, const char* opts_json
     PlanDev& pd = *e->plans[plan_id];
     if (in->ncols != pd.plan.in_schema.size()) return fail(e, TF_E_FATAL_ARG, "batch column count does not match the plan schema");
     if (in->nrows >= (1ull << 31)) return fail(e, TF_E_FATAL_ARG, "batch too large (>= 2^31 rows)");
-    try {
-        CK(cudaSetDevice(e->device));
+    return on_device(e, [&] {
         const uint64_t n = in->nrows;
         cudaStream_t s = e->stream;
-        try { dbz_build_template(pd, opts_json); } catch (const std::runtime_error& x) { return fail(e, TF_E_FATAL_CONFIG, std::string("opts_json: ") + x.what()); }
+        const tfj::ValuePtr ov = parse_opts_json(opts_json);
+        dbz_build_template(pd, opts_json, *ov);
         std::vector<tf_col> dev; const uint8_t* dev_kinds = stage_input(e, in, dev);
         e->dbz = pd.dbz;
-        const size_t o_id = 0, o_lsn = align_up(n * 4 + 16, 256), o_ct = o_lsn + align_up(n * 8 + 16, 256), o_off = o_ct + align_up(n * 8 + 16, 256), o_pre = o_off + align_up((n + 1) * 4 + 16, 256), o_heap = o_pre + align_up(n + 16, 256);
         uint64_t gt_len = 0;
         if (meta && in->mem == TF_MEM_HOST && meta->txid_offsets && meta->txid_heap) gt_len = meta->txid_offsets[n];
-        e->dbz_meta.ensure(o_heap + gt_len + 256);
+        Layout L(16);
+        const size_t o_id = L.take(n * 4), o_lsn = L.take(n * 8), o_ct = L.take(n * 8), o_off = L.take((n + 1) * 4), o_heap = L.take(gt_len);
+        e->dbz_meta.ensure(L.total() + 256);
         uint8_t* M = e->dbz_meta.p;
         if (meta) {
             if (in->mem == TF_MEM_HOST) {
@@ -1170,7 +1134,6 @@ int tfgpu_emit_debezium_crud(tfgpu_engine* e, int plan_id, const char* opts_json
         }
         // update / delete events: kinds + OldKeys (as a second set of typed columns) reach the row writer
         {
-            auto ov = tfj::parse(opts_json);
             const tfplan::Plan& pl = pd.plan; const size_t nc = pl.in_schema.size();
             e->dbz.kinds = dev_kinds; e->dbz.snapshot = ov->get_bool("snapshot") ? 1 : 0; e->dbz.mysql_src = ov->get_str("source_type") == "mysql" ? 1 : 0;
             const tfj::Value* tv = ov->get("tombstones_on_delete"); e->dbz.tombstones = (tv && tv->kind == tfj::Value::Bool && !tv->b) ? 0 : 1;      // tombstones.on.delete, default true
@@ -1182,15 +1145,15 @@ int tfgpu_emit_debezium_crud(tfgpu_engine* e, int plan_id, const char* opts_json
                 std::vector<tf_col> odev; stage_input(e, old->values, odev, &e->old_arena);
                 std::vector<DCol> oc(nc); std::vector<uint8_t> present(nc, 0); int np = 0;
                 for (size_t c = 0; c < nc; c++) {
-                    const tf_col& ic = odev[c]; DCol& d = oc[c]; std::memset(&d, 0, sizeof d);
+                    const tf_col& ic = odev[c];
                     if (ic.type != pl.in_schema[c].tf) return fail(e, TF_E_FATAL_ARG, "old keys: column " + std::to_string(c) + " type does not match the plan schema");
-                    d.type = ic.type; d.out_kind = OK_COPY; d.in_w = in_width(ic.type); d.out_w = d.in_w; d.str_slot = -1; d.mask_slot = -1;
-                    d.values = (const uint8_t*)ic.values; d.validity = ic.validity; d.offsets = ic.offsets; d.heap = ic.heap; d.aux = (const uint8_t*)ic.aux;
+                    DCol& d = oc[c]; d = make_dcol(ic, ic.type); d.out_kind = OK_COPY; d.out_w = d.in_w;
                     present[c] = (old->present_cols && old->present_cols[c]) ? 1 : 0; np += present[c];
                     if (present[c] && n) { if (d.in_w && !d.values) return fail(e, TF_E_FATAL_ARG, "old keys: values pointer is NULL"); if (!d.in_w && !d.offsets) return fail(e, TF_E_FATAL_ARG, "old keys: offsets pointer is NULL"); }
                 }
-                const size_t o_oc = 0, o_pr = align_up(nc * sizeof(DCol) + 16, 256), o_has = o_pr + align_up(nc + 16, 256);
-                e->dbz_old.ensure(o_has + n + 256);
+                Layout O(16);
+                const size_t o_oc = O.take(nc * sizeof(DCol)), o_pr = O.take(nc), o_has = O.take(n);
+                e->dbz_old.ensure(O.total() + 256);
                 CK(cudaMemcpyAsync(e->dbz_old.p + o_oc, oc.data(), nc * sizeof(DCol), cudaMemcpyHostToDevice, s));
                 CK(cudaMemcpyAsync(e->dbz_old.p + o_pr, present.data(), nc, cudaMemcpyHostToDevice, s));
                 e->dbz.old_cols = (const DCol*)(e->dbz_old.p + o_oc); e->dbz.old_present = e->dbz_old.p + o_pr; e->dbz.n_old_present = np;
@@ -1206,23 +1169,20 @@ int tfgpu_emit_debezium_crud(tfgpu_engine* e, int plan_id, const char* opts_json
         finish_wire(e, n, TF_WIRE_DEBEZIUM, r.get());
         *out = r.release();
         return TF_OK;
-    } catch (const tfplan::FatalError& f) { return fail(e, f.code, f.what()); }
-    catch (const CudaError& c) { return cuda_fail(e, c); }
-    catch (const std::bad_alloc&) { return fail(e, TF_E_RETRY_OOM, "host allocation failed"); }
+    });
 }
 
 // Measurer middleware (synchronizer/measurer.go:38-42): Size.Values of every row and their sum, in one pass over the columns.
 int tfgpu_measure(tfgpu_engine* e, const tf_batch* in, uint64_t* per_row, uint64_t* total) {
     if (!e || !in || !total) return TF_E_FATAL_ARG;
-    try {
-        CK(cudaSetDevice(e->device));
+    return on_device(e, [&] {
         cudaStream_t s = e->stream;
         join_tail(e);                     // the work arena is reused below
         std::vector<tf_col> dev; stage_input(e, in, dev);
         const size_t nc = in->ncols; const uint64_t n = in->nrows;
-        if (e->d_cols_cap < nc) { if (e->d_cols) CK(cudaFree(e->d_cols)); CK(cudaMalloc(&e->d_cols, sizeof(DCol) * (nc ? nc : 1))); e->d_cols_cap = nc; }
+        ensure_d_cols(e, nc);
         std::vector<DCol> hc(nc);
-        for (size_t c = 0; c < nc; c++) { const tf_col& ic = dev[c]; DCol& d = hc[c]; std::memset(&d, 0, sizeof d); d.type = ic.type; d.in_w = in_width(ic.type); d.values = (const uint8_t*)ic.values; d.validity = ic.validity; d.offsets = ic.offsets; d.heap = ic.heap; d.aux = (const uint8_t*)ic.aux; }
+        for (size_t c = 0; c < nc; c++) hc[c] = make_dcol(dev[c], dev[c].type);
         e->work.ensure(n * 8 + 256);
         unsigned long long* d_total = (unsigned long long*)e->work.p; uint64_t* d_rows = per_row ? (uint64_t*)(e->work.p + 64) : nullptr;
         CK(cudaMemcpyAsync(e->d_cols, hc.data(), sizeof(DCol) * nc, cudaMemcpyHostToDevice, s));
@@ -1233,10 +1193,62 @@ int tfgpu_measure(tfgpu_engine* e, const tf_batch* in, uint64_t* per_row, uint64
         if (per_row && n) CK(cudaMemcpyAsync(per_row, d_rows, n * 8, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
         return TF_OK;
-    } catch (const tfplan::FatalError& f) { return fail(e, f.code, f.what()); }
-    catch (const CudaError& c) { return cuda_fail(e, c); }
-    catch (const std::bad_alloc&) { return fail(e, TF_E_RETRY_OOM, "host allocation failed"); }
+    });
 }
+
+}  // extern "C"
+
+// ---------------------------------------------------------------------------------------------- parsers
+// What the three parsers (CSV, JSON lines, Debezium) share: their input text, argument checks and the chain over the staged batch.
+namespace {
+// wire_fmt of a parser: 0 (Transformed rows) or a format the encode entry points accept
+int check_wire_fmt(tfgpu_engine* e, const PlanDev& pd, int wire_fmt) {
+    if (wire_fmt != 0 && !wire_known(wire_fmt)) return fail(e, TF_E_FATAL_UNSUPPORTED, "wire format not implemented");
+    if (wire_fmt != 0 && !wire_is_ser(wire_fmt) && !pd.plan.has_sink) return fail(e, TF_E_FATAL_CONFIG, "plan was built without a sink");
+    return TF_OK;
+}
+
+// message `m` ends at end(m): the ends must be non-decreasing and the last one must be the end of the buffer
+template <typename End> int check_msg_ends(tfgpu_engine* e, uint32_t n_msgs, uint64_t len, End end) {
+    uint64_t prev = 0;
+    for (uint32_t m = 0; m < n_msgs; m++) { if (end(m) < prev || end(m) > len) return fail(e, TF_E_FATAL_ARG, "message ends must be non-decreasing and inside the buffer"); prev = end(m); }
+    if ((n_msgs ? end(n_msgs - 1) : 0) != len) return fail(e, TF_E_FATAL_ARG, "the messages must cover the whole buffer");
+    return TF_OK;
+}
+
+// the text in HBM: host bytes are copied to csv_text, device bytes are read in place
+const uint8_t* stage_text(tfgpu_engine* e, const uint8_t* bytes, uint64_t len, int mem) {
+    if (mem != TF_MEM_HOST) return bytes;
+    e->csv_text.ensure(len + 64);
+    if (len) CK(cudaMemcpyAsync(e->csv_text.p, bytes, len, cudaMemcpyHostToDevice, e->stream));
+    return e->csv_text.p;
+}
+
+// The staged columns (device resident, nrows rows) through the chain and out as wire_fmt asks. A row error whose term the parser left
+// open (0xff) takes the column the parser recorded for its row in d_errcol.
+std::unique_ptr<tfgpu_result> run_staged(tfgpu_engine* e, PlanDev& pd, std::vector<tf_col>& dev, uint64_t nrows, const uint8_t* kinds,
+                                         const uint8_t* pre_err, const uint8_t* d_errcol, int wire_fmt) {
+    const tf_batch staged{nrows, (uint32_t)dev.size(), TF_MEM_DEVICE, dev.data(), nullptr};
+    run_chain(e, pd, &staged, dev.data(), kinds, wire_fmt == 0 ? TF_WIRE_COLUMNAR_INTERNAL : wire_fmt, pre_err);
+    auto r = std::make_unique<tfgpu_result>();
+    if (wire_fmt == 0) finish_columnar(e, pd, nrows, r.get()); else finish_wire(e, nrows, wire_fmt, r.get());
+    if (d_errcol && !r->errs.empty()) {
+        std::vector<uint8_t> ecol(nrows);
+        CK(cudaMemcpyAsync(ecol.data(), d_errcol, nrows, cudaMemcpyDeviceToHost, e->stream)); CK(cudaStreamSynchronize(e->stream));
+        for (auto& x : r->errs) if (x.term == 0xff) x.term = ecol[x.row];
+    }
+    return r;
+}
+
+// A var-width column of a staged batch: its offsets are row `slot` of d_off [nslots][nrows+1], its text at its base in `heap`.
+void staged_text_col(tf_col& d, int slot, const uint8_t* d_off, uint64_t nrows, const uint8_t* heap, const Heaps& h) {
+    d.offsets = (const uint32_t*)d_off + (size_t)slot * (nrows + 1);
+    d.heap = heap ? heap + h.base[slot] : nullptr;
+    d.heap_len = heap ? h.total[slot] : 0;
+}
+}  // namespace
+
+extern "C" {
 
 // ---------------------------------------------------------------------------------------------- CSV
 // parsers.Parser for the S3 CSV source (pkg/providers/s3/reader/registry/csv/reader_csv.go:85-452) fused with the
@@ -1282,21 +1294,19 @@ int tfgpu_parse_csv(tfgpu_engine* e, int plan_id, const char* opts_json, const u
     *out = nullptr;
     PlanDev& pd = *e->plans[plan_id];
     if (len >= (1ull << 32) - 16) return fail(e, TF_E_FATAL_ARG, "csv chunk must be < 4 GiB (line positions are uint32)");
-    if (wire_fmt != 0 && !wire_known(wire_fmt)) return fail(e, TF_E_FATAL_UNSUPPORTED, "wire format not implemented");
-    if (wire_fmt != 0 && !wire_is_ser(wire_fmt) && !pd.plan.has_sink) return fail(e, TF_E_FATAL_CONFIG, "plan was built without a sink");
-    try {
-        CK(cudaSetDevice(e->device));
+    if (const int rc = check_wire_fmt(e, pd, wire_fmt)) return rc;
+    return on_device(e, [&] {
         cudaStream_t s = e->stream;
         CsvHostOpts ho = parse_csv_opts(opts_json);
         const tfplan::Plan& pl = pd.plan; const size_t nc = pl.in_schema.size();
-        // text into HBM
-        const uint8_t* d_text = bytes;
-        if (mem == TF_MEM_HOST) { e->csv_text.ensure(len + 64); if (len) CK(cudaMemcpyAsync(e->csv_text.p, bytes, len, cudaMemcpyHostToDevice, s)); d_text = e->csv_text.p; }
+        const uint8_t* d_text = stage_text(e, bytes, len, mem);
         // newline index
         const uint32_t nblk = (uint32_t)((len + CSV_NL_BLOCK - 1) / CSV_NL_BLOCK);
         uint64_t nlines = 0;
-        e->work.ensure(((size_t)nblk * 8 + 1024) * 2 + 4096);
-        uint32_t* blk_cnt = (uint32_t*)e->work.p; uint32_t* blk_off = blk_cnt + align_up(nblk + 1, 64);
+        Layout W;
+        const size_t w_cnt = W.take(((size_t)nblk + 1) * 4), w_off = W.take(((size_t)nblk + 64) * 4);
+        e->work.ensure(W.total() + 256);
+        uint32_t* blk_cnt = (uint32_t*)(e->work.p + w_cnt); uint32_t* blk_off = (uint32_t*)(e->work.p + w_off);
         if (nblk) {
             CK(cudaMemsetAsync(e->d_state, 0, sizeof(DState), s));
             e->prof_n = 0;
@@ -1308,30 +1318,29 @@ int tfgpu_parse_csv(tfgpu_engine* e, int plan_id, const char* opts_json, const u
         const uint64_t skip = ho.skip < nlines ? ho.skip : nlines;
         const uint64_t nrows = nlines - skip;
         // staging layout
-        std::vector<CsvColDev> hc(nc); std::vector<int16_t> next_same(nc, -1); int nfields = 0, nslots = 0, nany = 0;
+        std::vector<CsvColDev> hc(nc); std::vector<int16_t> next_same(nc, -1); int nfields = 0, nslots = 0;
         for (size_t c = 0; c < nc; c++) {
             const tfplan::ColSchema& cs = pl.in_schema[c]; CsvColDev& d = hc[c]; std::memset(&d, 0, sizeof d);
             d.tf = cs.tf; d.w = in_width(cs.tf); d.slot = -1;
             d.path = cs.path.empty() ? (int)c : atoi(cs.path.c_str());        // reader_csv.go:286 strconv.Atoi(col.Path)
             if (!cs.path.empty() && cs.path.find_first_not_of("-0123456789") != std::string::npos) throw tfplan::FatalError(TF_E_FATAL_CONFIG, "csv: column path '" + cs.path + "' is not an index");
             if (d.path >= 0 && d.path + 1 > nfields) nfields = d.path + 1;
-            if (!d.w) { d.slot = nslots++; if (cs.tf == TF_ANY) nany++; }
+            if (!d.w) d.slot = nslots++;
         }
         if (nfields > 32000) throw tfplan::FatalError(TF_E_FATAL_UNSUPPORTED, "csv: too many fields");
         std::vector<int16_t> field_col(nfields ? nfields : 1, -1);
         for (int c = (int)nc - 1; c >= 0; c--) if (hc[c].path >= 0) { next_same[c] = field_col[hc[c].path]; field_col[hc[c].path] = (int16_t)c; }
-        size_t sb = 0; auto need = [&](size_t b) { size_t at = sb; sb += align_up(b ? b : 1, 256); return at; };
-        const size_t o_line = need((nlines + 1) * 4), o_err = need(nrows), o_cols = need(nc * sizeof(CsvColDev)), o_fc = need(field_col.size() * 2), o_ns = need(nc * 2),
-                     o_blob = need(ho.blob.size()), o_ss = need((size_t)nslots * nrows * 4), o_sl = need((size_t)nslots * nrows * 4),
-                     o_off = need((size_t)nslots * (nrows + 1) * 4), o_tot = need((size_t)nslots * 8 + 8), o_base = need((size_t)nslots * 8 + 8);
+        Layout L;
+        const size_t o_line = L.take((nlines + 1) * 4), o_err = L.take(nrows), o_cols = L.take(nc * sizeof(CsvColDev)), o_fc = L.take(field_col.size() * 2), o_ns = L.take(nc * 2),
+                     o_blob = L.take(ho.blob.size()), o_ss = L.take((size_t)nslots * nrows * 4), o_sl = L.take((size_t)nslots * nrows * 4),
+                     o_off = L.take((size_t)nslots * (nrows + 1) * 4), o_tot = L.take((size_t)nslots * 8 + 8), o_base = L.take((size_t)nslots * 8 + 8);
         std::vector<size_t> o_val(nc), o_aux(nc);
         for (size_t c = 0; c < nc; c++) {
-            o_val[c] = hc[c].w ? need((size_t)hc[c].w * nrows) : 0;
+            o_val[c] = hc[c].w ? L.take((size_t)hc[c].w * nrows) : 0;
             const int tf = hc[c].tf;
-            o_aux[c] = (tf == TF_DATE || tf == TF_DATETIME || tf == TF_TIMESTAMP) ? need(4 * nrows) : (tf == TF_ANY ? need(nrows) : 0);
+            o_aux[c] = (tf == TF_DATE || tf == TF_DATETIME || tf == TF_TIMESTAMP) ? L.take(4 * nrows) : (tf == TF_ANY ? L.take(nrows) : 0);
         }
-        const size_t o_heap = need(len + 2 * nrows * (size_t)(nany ? nany : 0) + 64);
-        e->csv_stage.ensure(sb + 256);
+        e->csv_stage.ensure(L.total() + 256);
         uint8_t* B = e->csv_stage.p;
         for (size_t c = 0; c < nc; c++) {
             if (hc[c].w) hc[c].values = B + o_val[c];
@@ -1343,18 +1352,18 @@ int tfgpu_parse_csv(tfgpu_engine* e, int plan_id, const char* opts_json, const u
         CK(cudaMemcpyAsync(B + o_fc, field_col.data(), field_col.size() * 2, cudaMemcpyHostToDevice, s));
         CK(cudaMemcpyAsync(B + o_ns, next_same.data(), nc * 2, cudaMemcpyHostToDevice, s));
         CK(cudaMemcpyAsync(B + o_blob, ho.blob.data(), ho.blob.size(), cudaMemcpyHostToDevice, s));
-        std::vector<uint64_t> col_total(nslots ? nslots : 1, 0), col_base(nslots ? nslots : 1, 0);
+        Heaps h; const uint8_t* heap = nullptr;
         if (nlines) { e->prof_begin("k_csv_line_index", s); launch_k_csv_line_index(nblk, 256, 0, s, d_text, len, blk_off, (uint32_t*)(B + o_line), nullptr); e->prof_end(s); }
         if (nrows) {
             CsvArgs ca{d_text, len, (const uint32_t*)(B + o_line), nlines, skip, ho.cfg, B + o_blob, (const CsvColDev*)(B + o_cols), (int)nc,
                        (const int16_t*)(B + o_fc), nfields, (const int16_t*)(B + o_ns), (uint32_t*)(B + o_ss), (uint32_t*)(B + o_sl), B + o_err};
             e->prof_begin("k_csv_pass1", s); launch_k_csv_pass1((uint32_t)std::min<uint64_t>((nrows + CSV_TILE_ROWS - 1) / CSV_TILE_ROWS, (uint64_t)e->sm_count * 16), 32 * CSV_WARPS, 0, s, ca); e->prof_end(s);
             if (nslots) {
-                launch_offsets(e, (const uint32_t*)(B + o_sl), nrows, (uint32_t)nslots, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), s);
-                CK(cudaMemcpyAsync(col_total.data(), B + o_tot, (size_t)nslots * 8, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
-                uint64_t run = 0; for (int k = 0; k < nslots; k++) { col_base[k] = run; run += col_total[k]; }
-                CK(cudaMemcpyAsync(B + o_base, col_base.data(), (size_t)nslots * 8, cudaMemcpyHostToDevice, s));
-                CsvCopyArgs cp{d_text, (const uint32_t*)(B + o_ss), (const uint32_t*)(B + o_sl), (const uint32_t*)(B + o_off), B + o_heap, (const uint64_t*)(B + o_base), nrows};
+                // text heaps (the staged batch lives in csv_stage, in_arena is free)
+                h = size_heaps(e, (const uint32_t*)(B + o_sl), nrows, (uint32_t)nslots, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), (uint64_t*)(B + o_base),
+                               e->in_arena, "csv chunk: a text column exceeds 4 GiB");
+                heap = e->in_arena.p;
+                CsvCopyArgs cp{d_text, (const uint32_t*)(B + o_ss), (const uint32_t*)(B + o_sl), (const uint32_t*)(B + o_off), e->in_arena.p, (const uint64_t*)(B + o_base), nrows};
                 e->prof_begin("k_csv_pass2", s); launch_k_csv_pass2(dim3((uint32_t)((nrows + 255) / 256), nslots), 256, 0, s, cp); e->prof_end(s);
             }
         }
@@ -1363,23 +1372,15 @@ int tfgpu_parse_csv(tfgpu_engine* e, int plan_id, const char* opts_json, const u
         for (size_t c = 0; c < nc; c++) {
             tf_col& d = dev[c]; std::memset(&d, 0, sizeof d); d.type = hc[c].tf;
             if (hc[c].w) { d.values = hc[c].values; d.aux = hc[c].aux32; }
-            else { d.offsets = (const uint32_t*)(B + o_off) + (size_t)hc[c].slot * (nrows + 1); d.heap = B + o_heap + col_base[hc[c].slot]; d.heap_len = col_total[hc[c].slot]; d.aux = hc[c].aux8; }
+            else { staged_text_col(d, hc[c].slot, B + o_off, nrows, heap, h); d.aux = hc[c].aux8; }
         }
-        tf_batch staged; staged.nrows = nrows; staged.ncols = (uint32_t)nc; staged.mem = TF_MEM_DEVICE; staged.cols = dev.data(); staged.kinds = nullptr;
-        const int saved_prof = e->prof_n;
-        run_chain(e, pd, &staged, dev.data(), nullptr, wire_fmt == 0 ? TF_WIRE_COLUMNAR_INTERNAL : wire_fmt, nrows ? B + o_err : nullptr);
-        (void)saved_prof;
-        auto r = std::make_unique<tfgpu_result>();
-        if (wire_fmt == 0) finish_columnar(e, pd, nrows, r.get()); else finish_wire(e, nrows, wire_fmt, r.get());
+        auto r = run_staged(e, pd, dev, nrows, nullptr, nrows ? B + o_err : nullptr, nullptr, wire_fmt);
         uint32_t last_end = 0;
         if (nlines) { CK(cudaMemcpyAsync(&last_end, (uint32_t*)(B + o_line) + (nlines - 1), 4, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s)); }
         r->consumed = last_end;
         *out = r.release();
         return TF_OK;
-    } catch (const tfplan::FatalError& f) { return fail(e, f.code, f.what()); }
-    catch (const CudaError& c) { return cuda_fail(e, c); }
-    catch (const std::bad_alloc&) { return fail(e, TF_E_RETRY_OOM, "host allocation failed"); }
-    catch (const std::exception& x) { return fail(e, TF_E_FATAL_CONFIG, x.what()); }
+    });
 }
 
 // ---------------------------------------------------------------------------------------------- JSON lines
@@ -1391,12 +1392,9 @@ int tfgpu_parse_json(tfgpu_engine* e, int plan_id, const char* opts_json, const 
     *out = nullptr;
     PlanDev& pd = *e->plans[plan_id];
     if (len >= (1ull << 32) - 16) return fail(e, TF_E_FATAL_ARG, "json batch must be < 4 GiB (line positions are uint32)");
-    if (wire_fmt != 0 && !wire_known(wire_fmt)) return fail(e, TF_E_FATAL_UNSUPPORTED, "wire format not implemented");
-    if (wire_fmt != 0 && !wire_is_ser(wire_fmt) && !pd.plan.has_sink) return fail(e, TF_E_FATAL_CONFIG, "plan was built without a sink");
-    { uint64_t prev = 0; for (uint32_t m = 0; m < n_msgs; m++) { if (msgs[m].end < prev || msgs[m].end > len) return fail(e, TF_E_FATAL_ARG, "message ends must be non-decreasing and inside the buffer"); prev = msgs[m].end; }
-      if ((n_msgs ? msgs[n_msgs - 1].end : 0) != len) return fail(e, TF_E_FATAL_ARG, "the messages must cover the whole buffer"); }
-    try {
-        CK(cudaSetDevice(e->device));
+    if (const int rc = check_wire_fmt(e, pd, wire_fmt)) return rc;
+    if (const int rc = check_msg_ends(e, n_msgs, len, [&](uint32_t m) { return msgs[m].end; })) return rc;
+    return on_device(e, [&] {
         cudaStream_t s = e->stream;
         const tfplan::Plan& pl = pd.plan; const size_t nc = pl.in_schema.size();
         // ---- options (AuxParserOpts, generic_parser.go:41-84)
@@ -1434,17 +1432,16 @@ int tfgpu_parse_json(tfgpu_engine* e, int plan_id, const char* opts_json, const 
         }
         const uint32_t part_off = (uint32_t)names.size(); names.insert(names.end(), partition.begin(), partition.end());
         // ---- text and message table into HBM
-        const uint8_t* d_text = bytes;
-        if (mem == TF_MEM_HOST) { e->csv_text.ensure(len + 64); if (len) CK(cudaMemcpyAsync(e->csv_text.p, bytes, len, cudaMemcpyHostToDevice, s)); d_text = e->csv_text.p; }
+        const uint8_t* d_text = stage_text(e, bytes, len, mem);
         const uint32_t nblk = (uint32_t)((len + CSV_NL_BLOCK - 1) / CSV_NL_BLOCK);
         const size_t bits_words = (size_t)(len / 32 + 2);
         std::vector<uint64_t> h_end(n_msgs ? n_msgs : 1), h_off(n_msgs ? n_msgs : 1); std::vector<int64_t> h_ws(n_msgs ? n_msgs : 1); std::vector<uint32_t> h_wn(n_msgs ? n_msgs : 1);
         for (uint32_t m = 0; m < n_msgs; m++) { h_end[m] = msgs[m].end; h_off[m] = msgs[m].offset; h_ws[m] = msgs[m].write_sec; h_wn[m] = msgs[m].write_nsec; }
         {
-            size_t wb = 0; auto need = [&](size_t b) { size_t at = wb; wb += align_up(b ? b : 1, 256); return at; };
-            const size_t w_cnt = need(((size_t)nblk + 64) * 4), w_off = need(((size_t)nblk + 64) * 4), w_bits = need(bits_words * 4),
-                         w_end = need((size_t)n_msgs * 8), w_moff = need((size_t)n_msgs * 8), w_ws = need((size_t)n_msgs * 8), w_wn = need((size_t)n_msgs * 4), w_r0 = need((size_t)n_msgs * 4);
-            e->json_msgs.ensure(wb + 256);                       // message table + line-count scratch live here until the text heap is sized
+            Layout M;
+            const size_t w_cnt = M.take(((size_t)nblk + 64) * 4), w_off = M.take(((size_t)nblk + 64) * 4), w_bits = M.take(bits_words * 4),
+                         w_end = M.take((size_t)n_msgs * 8), w_moff = M.take((size_t)n_msgs * 8), w_ws = M.take((size_t)n_msgs * 8), w_wn = M.take((size_t)n_msgs * 4), w_r0 = M.take((size_t)n_msgs * 4);
+            e->json_msgs.ensure(M.total() + 256);                // message table + line-count scratch live here until the text heap is sized
             uint8_t* W = e->json_msgs.p;
             uint32_t* blk_cnt = (uint32_t*)(W + w_cnt); uint32_t* blk_off = (uint32_t*)(W + w_off); uint32_t* endbits = (uint32_t*)(W + w_bits);
             uint64_t nlines = 0;
@@ -1462,20 +1459,20 @@ int tfgpu_parse_json(tfgpu_engine* e, int plan_id, const char* opts_json, const 
             }
             const uint64_t nrows = nlines;
             // ---- staging layout (csv_stage arena)
-            size_t sb = 0; auto sneed = [&](size_t b) { size_t at = sb; sb += align_up(b ? b : 1, 256); return at; };
+            Layout L;
             const uint32_t nlb = (uint32_t)((nlines + 127) / 128);
-            const size_t o_line = sneed((nlines + 1) * 4), o_rank = sneed((nlines + 2) * 4), o_lcnt = sneed(((size_t)nlb + 64) * 4), o_loff = sneed(((size_t)nlb + 64) * 4),
-                         o_err = sneed(nrows), o_ecol = sneed(nrows), o_cols = sneed(nc * sizeof(JsnColDev)), o_names = sneed(names.size()),
-                         o_ss = sneed((size_t)nf * nrows * 4), o_sl = sneed((size_t)nf * nrows * 4), o_len = sneed((size_t)nslots * nrows * 4),
-                         o_off = sneed((size_t)nslots * (nrows + 1) * 4), o_tot = sneed((size_t)nslots * 8 + 8), o_base = sneed((size_t)nslots * 8 + 8);
+            const size_t o_line = L.take((nlines + 1) * 4), o_rank = L.take((nlines + 2) * 4), o_lcnt = L.take(((size_t)nlb + 64) * 4), o_loff = L.take(((size_t)nlb + 64) * 4),
+                         o_err = L.take(nrows), o_ecol = L.take(nrows), o_cols = L.take(nc * sizeof(JsnColDev)), o_names = L.take(names.size()),
+                         o_ss = L.take((size_t)nf * nrows * 4), o_sl = L.take((size_t)nf * nrows * 4), o_len = L.take((size_t)nslots * nrows * 4),
+                         o_off = L.take((size_t)nslots * (nrows + 1) * 4), o_tot = L.take((size_t)nslots * 8 + 8), o_base = L.take((size_t)nslots * 8 + 8);
             std::vector<size_t> o_val(nc), o_aux(nc), o_vld(nc);
             for (size_t c = 0; c < nc; c++) {
-                o_val[c] = hc[c].w ? sneed((size_t)hc[c].w * nrows) : 0;
+                o_val[c] = hc[c].w ? L.take((size_t)hc[c].w * nrows) : 0;
                 const int tf = hc[c].tf;
-                o_aux[c] = (tf == TF_DATE || tf == TF_DATETIME || tf == TF_TIMESTAMP) ? sneed(4 * nrows) : (tf == TF_ANY ? sneed(nrows) : 0);
-                o_vld[c] = sneed((nrows / 32 + 2) * 4);
+                o_aux[c] = (tf == TF_DATE || tf == TF_DATETIME || tf == TF_TIMESTAMP) ? L.take(4 * nrows) : (tf == TF_ANY ? L.take(nrows) : 0);
+                o_vld[c] = L.take((nrows / 32 + 2) * 4);
             }
-            e->csv_stage.ensure(sb + 256);
+            e->csv_stage.ensure(L.total() + 256);
             uint8_t* B = e->csv_stage.p;
             for (size_t c = 0; c < nc; c++) {
                 if (hc[c].w) hc[c].values = B + o_val[c];
@@ -1484,9 +1481,8 @@ int tfgpu_parse_json(tfgpu_engine* e, int plan_id, const char* opts_json, const 
                 if (tf == TF_ANY) hc[c].aux8 = B + o_aux[c];
                 hc[c].validity = (uint32_t*)(B + o_vld[c]);
             }
-            std::vector<uint64_t> col_total(nslots ? nslots : 1, 0), col_base(nslots ? nslots : 1, 0);
+            Heaps h; const uint8_t* heap = nullptr;
             uint32_t n_nonempty = 0;
-            const uint8_t* heap = nullptr;
             if (nrows) {
                 CK(cudaMemcpyAsync(B + o_cols, hc.data(), nc * sizeof(JsnColDev), cudaMemcpyHostToDevice, s));
                 CK(cudaMemcpyAsync(B + o_names, names.data(), names.size(), cudaMemcpyHostToDevice, s));
@@ -1508,13 +1504,10 @@ int tfgpu_parse_json(tfgpu_engine* e, int plan_id, const char* opts_json, const 
                 e->prof_begin("k_json_pass1", s); launch_k_json_pass1(nlb, 128, JSN_STAGE, s, ja); e->prof_end(s);
                 CK(cudaMemcpyAsync(&n_nonempty, (uint32_t*)(B + o_rank) + nlines, 4, cudaMemcpyDeviceToHost, s));
                 if (nslots) {
-                    launch_offsets(e, (const uint32_t*)(B + o_len), nrows, (uint32_t)nslots, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), s);
-                    CK(cudaMemcpyAsync(col_total.data(), B + o_tot, (size_t)nslots * 8, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
-                    uint64_t run = 0; for (int k = 0; k < nslots; k++) { col_base[k] = run; run += align_up(col_total[k], 16); }
-                    if (run >= (1ull << 32)) throw tfplan::FatalError(TF_E_FATAL_ARG, "json batch: a text column exceeds 4 GiB");
-                    e->in_arena.ensure(run + 256);               // text heaps (the staged batch is device resident, in_arena is free)
+                    // text heaps (the staged batch is device resident, in_arena is free)
+                    h = size_heaps(e, (const uint32_t*)(B + o_len), nrows, (uint32_t)nslots, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), (uint64_t*)(B + o_base),
+                                   e->in_arena, "json batch: a text column exceeds 4 GiB");
                     heap = e->in_arena.p;
-                    CK(cudaMemcpyAsync(B + o_base, col_base.data(), (size_t)nslots * 8, cudaMemcpyHostToDevice, s));
                     JsnWriteArgs wa{ja, (const uint32_t*)(B + o_off), e->in_arena.p, (const uint64_t*)(B + o_base)};
                     e->prof_begin("k_json_pass2", s); launch_k_json_pass2(nlb, 128, JSN_STAGE, s, wa); e->prof_end(s);
                 } else CK(cudaStreamSynchronize(s));
@@ -1524,28 +1517,19 @@ int tfgpu_parse_json(tfgpu_engine* e, int plan_id, const char* opts_json, const 
             for (size_t c = 0; c < nc; c++) {
                 tf_col& d = dev[c]; std::memset(&d, 0, sizeof d); d.type = hc[c].tf; d.validity = (const uint8_t*)hc[c].validity;
                 if (hc[c].w) { d.values = hc[c].values; d.aux = hc[c].aux32; }
-                else { d.offsets = (const uint32_t*)(B + o_off) + (size_t)hc[c].slot * (nrows + 1); d.heap = heap ? heap + col_base[hc[c].slot] : nullptr; d.heap_len = col_total[hc[c].slot]; d.aux = hc[c].aux8; }
+                else { staged_text_col(d, hc[c].slot, B + o_off, nrows, heap, h); d.aux = hc[c].aux8; }
             }
-            tf_batch staged; staged.nrows = nrows; staged.ncols = (uint32_t)nc; staged.mem = TF_MEM_DEVICE; staged.cols = dev.data(); staged.kinds = nullptr;
-            run_chain(e, pd, &staged, dev.data(), nullptr, wire_fmt == 0 ? TF_WIRE_COLUMNAR_INTERNAL : wire_fmt, nrows ? B + o_err : nullptr);
-            auto r = std::make_unique<tfgpu_result>();
-            if (wire_fmt == 0) finish_columnar(e, pd, nrows, r.get()); else finish_wire(e, nrows, wire_fmt, r.get());
-            // row errors: row = index among the NON-EMPTY lines (empty lines are not lines to the reference, :528-530), term = column
-            if (!r->errs.empty()) {
-                std::vector<uint8_t> ecol(nrows); CK(cudaMemcpyAsync(ecol.data(), B + o_ecol, nrows, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
-                std::vector<tf_rowerr> keep; uint32_t empties = 0;
-                for (auto& x : r->errs) { if (x.code == JSN_EMPTY) { empties++; continue; } tf_rowerr y = x; if (y.term == 0xff) y.term = ecol[x.row]; y.row = x.row - empties; keep.push_back(y); }
-                r->errs.swap(keep);
-            }
+            auto r = run_staged(e, pd, dev, nrows, nullptr, nrows ? B + o_err : nullptr, B + o_ecol, wire_fmt);
+            // row errors: row = index among the NON-EMPTY lines (empty lines are not lines to the reference, :528-530)
+            std::vector<tf_rowerr> keep; uint32_t empties = 0;
+            for (const tf_rowerr& x : r->errs) { if (x.code == JSN_EMPTY) { empties++; continue; } keep.push_back(x); keep.back().row -= empties; }
+            r->errs.swap(keep);
             r->rows_in = n_nonempty;
             r->consumed = len;
             *out = r.release();
         }
         return TF_OK;
-    } catch (const tfplan::FatalError& f) { return fail(e, f.code, f.what()); }
-    catch (const CudaError& c) { return cuda_fail(e, c); }
-    catch (const std::bad_alloc&) { return fail(e, TF_E_RETRY_OOM, "host allocation failed"); }
-    catch (const std::exception& x) { return fail(e, TF_E_FATAL_CONFIG, x.what()); }
+    });
 }
 
 // ---------------------------------------------------------------------------------------------- Debezium
@@ -1577,18 +1561,23 @@ std::vector<DbzHostField> dbz_fields(const tfj::Value& schema, const char* which
     }
     return out;
 }
+
+// the table of an envelope schema: the fields of its `after` struct, which `before` must repeat
+std::vector<DbzHostField> dbz_table_fields(const tfj::Value& schema) {
+    const std::vector<DbzHostField> fs = dbz_fields(schema, "after"), fb = dbz_fields(schema, "before");
+    bool same = fs.size() == fb.size();
+    for (size_t i = 0; same && i < fs.size(); i++) same = fs[i].name == fb[i].name && fs[i].recv == fb[i].recv && fs[i].scale == fb[i].scale;
+    if (!same) throw tfplan::FatalError(TF_E_FATAL_UNSUPPORTED, "debezium: 'before' and 'after' structs differ");
+    return fs;
+}
 }  // namespace
 
 // Host-only: the table schema and receivers tfgpu_parse_debezium derives from a Kafka Connect envelope schema (no GPU needed):
 // [{"name","type","key","recv","scale"}, ...] in the order of the `after` struct, or the error the call would return.
 int tfgpu_debezium_schema_validate(const char* schema_text, char* describe_out, uint64_t cap, char* err_out, uint64_t err_cap) {
-    auto put = [](char* dst, uint64_t cap_, const std::string& s) { if (dst && cap_) { size_t n = s.size() < cap_ - 1 ? s.size() : cap_ - 1; std::memcpy(dst, s.data(), n); dst[n] = 0; } };
     if (!schema_text) return TF_E_FATAL_ARG;
-    try {
-        auto sv = tfj::parse(schema_text);
-        const std::vector<DbzHostField> fs = dbz_fields(*sv, "after"), fb = dbz_fields(*sv, "before");
-        if (fs.size() != fb.size()) throw tfplan::FatalError(TF_E_FATAL_UNSUPPORTED, "debezium: 'before' and 'after' structs differ");
-        for (size_t i = 0; i < fs.size(); i++) if (fs[i].name != fb[i].name || fs[i].recv != fb[i].recv || fs[i].scale != fb[i].scale) throw tfplan::FatalError(TF_E_FATAL_UNSUPPORTED, "debezium: 'before' and 'after' structs differ");
+    return host_validate(describe_out, cap, err_out, err_cap, [&] {
+        const std::vector<DbzHostField> fs = dbz_table_fields(*tfj::parse(schema_text));
         static const char* yt[] = {"", "int8", "int16", "int32", "int64", "uint8", "uint16", "uint32", "uint64", "float", "double", "boolean", "string", "utf8", "any", "date", "datetime", "timestamp", "interval"};
         std::string d = "[";
         for (size_t i = 0; i < fs.size(); i++) {
@@ -1597,11 +1586,8 @@ int tfgpu_debezium_schema_validate(const char* schema_text, char* describe_out, 
                  ",\"recv\":" + std::to_string(fs[i].recv) + ",\"scale\":" + std::to_string(fs[i].scale) + "}";
         }
         d += "]";
-        if (describe_out && d.size() + 1 > cap) { put(err_out, err_cap, "describe buffer too small"); return TF_E_FATAL_ARG; }
-        put(describe_out, cap, d);
-        return TF_OK;
-    } catch (const tfplan::FatalError& f) { put(err_out, err_cap, f.what()); return f.code; }
-    catch (const std::exception& x) { put(err_out, err_cap, x.what()); return TF_E_FATAL_CONFIG; }
+        return d;
+    });
 }
 
 int tfgpu_parse_debezium(tfgpu_engine* e, int plan_id, const char* opts_json, const uint8_t* bytes, uint64_t len, int mem,
@@ -1610,12 +1596,9 @@ int tfgpu_parse_debezium(tfgpu_engine* e, int plan_id, const char* opts_json, co
     *out = nullptr;
     PlanDev& pd = *e->plans[plan_id];
     if (len >= (1ull << 32) - 16) return fail(e, TF_E_FATAL_ARG, "debezium batch must be < 4 GiB");
-    if (wire_fmt != 0 && !wire_known(wire_fmt)) return fail(e, TF_E_FATAL_UNSUPPORTED, "wire format not implemented");
-    if (wire_fmt != 0 && !wire_is_ser(wire_fmt) && !pd.plan.has_sink) return fail(e, TF_E_FATAL_CONFIG, "plan was built without a sink");
-    { uint64_t prev = 0; for (uint32_t m = 0; m < n_msgs; m++) { if (msg_ends[m] < prev || msg_ends[m] > len) return fail(e, TF_E_FATAL_ARG, "message ends must be non-decreasing and inside the buffer"); prev = msg_ends[m]; }
-      if ((n_msgs ? msg_ends[n_msgs - 1] : 0) != len) return fail(e, TF_E_FATAL_ARG, "the messages must cover the whole buffer"); }
-    try {
-        CK(cudaSetDevice(e->device));
+    if (const int rc = check_wire_fmt(e, pd, wire_fmt)) return rc;
+    if (const int rc = check_msg_ends(e, n_msgs, len, [&](uint32_t m) { return msg_ends[m]; })) return rc;
+    return on_device(e, [&] {
         cudaStream_t s = e->stream;
         const tfplan::Plan& pl = pd.plan; const size_t nc = pl.in_schema.size();
         auto ov = tfj::parse(opts_json);
@@ -1623,10 +1606,7 @@ int tfgpu_parse_debezium(tfgpu_engine* e, int plan_id, const char* opts_json, co
         const bool use_sr = ov->get_bool("schema_registry"), check_table = ov->get_bool("check_table");
         const uint32_t schema_id = (uint32_t)ov->get_num("schema_id", 0);
         if (schema_text.empty()) throw tfplan::FatalError(TF_E_FATAL_CONFIG, "debezium: opts.schema_text (the Kafka Connect schema this plan was built for) is required");
-        auto sv = tfj::parse(schema_text.c_str());
-        const std::vector<DbzHostField> fs = dbz_fields(*sv, "after"), fb = dbz_fields(*sv, "before");
-        if (fs.size() != fb.size()) throw tfplan::FatalError(TF_E_FATAL_UNSUPPORTED, "debezium: 'before' and 'after' structs differ");
-        for (size_t i = 0; i < fs.size(); i++) if (fs[i].name != fb[i].name || fs[i].recv != fb[i].recv || fs[i].scale != fb[i].scale) throw tfplan::FatalError(TF_E_FATAL_UNSUPPORTED, "debezium: 'before' and 'after' structs differ");
+        const std::vector<DbzHostField> fs = dbz_table_fields(*tfj::parse(schema_text));
         if (fs.size() != nc || nc > JSN_MAX_COLS) throw tfplan::FatalError(TF_E_FATAL_CONFIG, "debezium: the plan schema must be the table schema of the 'after' struct (at most 128 columns)");
         std::vector<DbzColDev> hc(nc); std::vector<uint8_t> names; int nslots = 0;
         for (size_t c = 0; c < nc; c++) {
@@ -1640,20 +1620,18 @@ int tfgpu_parse_debezium(tfgpu_engine* e, int plan_id, const char* opts_json, co
         const uint32_t ts_off = (uint32_t)names.size(); names.insert(names.end(), pl.ns.begin(), pl.ns.end());
         const uint32_t tn_off = (uint32_t)names.size(); names.insert(names.end(), pl.name.begin(), pl.name.end());
         const uint32_t st_off = (uint32_t)names.size(); names.insert(names.end(), schema_text.begin(), schema_text.end());
-        const uint8_t* d_text = bytes;
-        if (mem == TF_MEM_HOST) { e->csv_text.ensure(len + 64); if (len) CK(cudaMemcpyAsync(e->csv_text.p, bytes, len, cudaMemcpyHostToDevice, s)); d_text = e->csv_text.p; }
+        const uint8_t* d_text = stage_text(e, bytes, len, mem);
         const uint64_t n = n_msgs;
-        size_t sb = 0; auto need = [&](size_t b) { size_t at = sb; sb += align_up(b ? b : 1, 256); return at; };
-        const size_t o_end = need(n * 8), o_err = need(n), o_ecol = need(n), o_cols = need(nc * sizeof(DbzColDev)), o_names = need(names.size()),
-                     o_ss = need(nc * n * 4), o_sl = need(nc * n * 4), o_len = need((size_t)nslots * n * 4), o_off = need((size_t)nslots * (n + 1) * 4),
-                     o_tot = need((size_t)nslots * 8 + 8), o_base = need((size_t)nslots * 8 + 8), o_kind = need(n), o_tx = need(n * 4), o_lsn = need(n * 8), o_ct = need(n * 8);
+        Layout L;
+        const size_t o_end = L.take(n * 8), o_err = L.take(n), o_ecol = L.take(n), o_cols = L.take(nc * sizeof(DbzColDev)), o_names = L.take(names.size()),
+                     o_ss = L.take(nc * n * 4), o_sl = L.take(nc * n * 4), o_len = L.take((size_t)nslots * n * 4), o_off = L.take((size_t)nslots * (n + 1) * 4),
+                     o_tot = L.take((size_t)nslots * 8 + 8), o_base = L.take((size_t)nslots * 8 + 8), o_kind = L.take(n), o_tx = L.take(n * 4), o_lsn = L.take(n * 8), o_ct = L.take(n * 8);
         std::vector<size_t> o_val(nc), o_vld(nc);
-        for (size_t c = 0; c < nc; c++) { o_val[c] = hc[c].w ? need((size_t)hc[c].w * n) : 0; o_vld[c] = need((n / 32 + 2) * 4); }
-        e->csv_stage.ensure(sb + 256);
+        for (size_t c = 0; c < nc; c++) { o_val[c] = hc[c].w ? L.take((size_t)hc[c].w * n) : 0; o_vld[c] = L.take((n / 32 + 2) * 4); }
+        e->csv_stage.ensure(L.total() + 256);
         uint8_t* B = e->csv_stage.p;
         for (size_t c = 0; c < nc; c++) { if (hc[c].w) hc[c].values = B + o_val[c]; hc[c].validity = (uint32_t*)(B + o_vld[c]); }
-        std::vector<uint64_t> col_total(nslots ? nslots : 1, 0), col_base(nslots ? nslots : 1, 0);
-        const uint8_t* heap = nullptr;
+        Heaps h; const uint8_t* heap = nullptr;
         e->prof_n = 0;
         if (n) {
             CK(cudaMemcpyAsync(B + o_end, msg_ends, n * 8, cudaMemcpyHostToDevice, s));
@@ -1669,12 +1647,9 @@ int tfgpu_parse_debezium(tfgpu_engine* e, int plan_id, const char* opts_json, co
             const uint32_t nb = (uint32_t)((n + 127) / 128);
             e->prof_begin("k_dbz_pass1", s); launch_k_dbz_pass1(nb, 128, DBZ_STAGE, s, da); e->prof_end(s);
             if (nslots) {
-                launch_offsets(e, (const uint32_t*)(B + o_len), n, (uint32_t)nslots, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), s);
-                CK(cudaMemcpyAsync(col_total.data(), B + o_tot, (size_t)nslots * 8, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
-                uint64_t run = 0; for (int k = 0; k < nslots; k++) { col_base[k] = run; run += align_up(col_total[k], 16); }
-                if (run >= (1ull << 32)) throw tfplan::FatalError(TF_E_FATAL_ARG, "debezium batch: a text column exceeds 4 GiB");
-                e->in_arena.ensure(run + 256); heap = e->in_arena.p;
-                CK(cudaMemcpyAsync(B + o_base, col_base.data(), (size_t)nslots * 8, cudaMemcpyHostToDevice, s));
+                h = size_heaps(e, (const uint32_t*)(B + o_len), n, (uint32_t)nslots, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), (uint64_t*)(B + o_base),
+                               e->in_arena, "debezium batch: a text column exceeds 4 GiB");
+                heap = e->in_arena.p;
                 DbzWriteArgs wa{da, (const uint32_t*)(B + o_off), e->in_arena.p, (const uint64_t*)(B + o_base)};
                 e->prof_begin("k_dbz_pass2", s); launch_k_dbz_pass2(nb, 128, 0, s, wa); e->prof_end(s);
             }
@@ -1684,14 +1659,10 @@ int tfgpu_parse_debezium(tfgpu_engine* e, int plan_id, const char* opts_json, co
         for (size_t c = 0; c < nc; c++) {
             tf_col& d = dev[c]; std::memset(&d, 0, sizeof d); d.type = hc[c].tf; d.validity = (const uint8_t*)hc[c].validity;
             if (hc[c].w) d.values = hc[c].values;
-            else { d.offsets = (const uint32_t*)(B + o_off) + (size_t)hc[c].slot * (n + 1); d.heap = heap ? heap + col_base[hc[c].slot] : nullptr; d.heap_len = col_total[hc[c].slot]; }
+            else staged_text_col(d, hc[c].slot, B + o_off, n, heap, h);
         }
-        tf_batch staged; staged.nrows = n; staged.ncols = (uint32_t)nc; staged.mem = TF_MEM_DEVICE; staged.cols = dev.data(); staged.kinds = nullptr;
-        run_chain(e, pd, &staged, dev.data(), n ? B + o_kind : nullptr, wire_fmt == 0 ? TF_WIRE_COLUMNAR_INTERNAL : wire_fmt, n ? B + o_err : nullptr);
-        auto r = std::make_unique<tfgpu_result>();
-        if (wire_fmt == 0) finish_columnar(e, pd, n, r.get()); else finish_wire(e, n, wire_fmt, r.get());
+        auto r = run_staged(e, pd, dev, n, n ? B + o_kind : nullptr, n ? B + o_err : nullptr, B + o_ecol, wire_fmt);
         if (n) {
-            if (!r->errs.empty()) { std::vector<uint8_t> ecol(n); CK(cudaMemcpyAsync(ecol.data(), B + o_ecol, n, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s)); for (auto& x : r->errs) if (x.term == 0xff) x.term = ecol[x.row]; }
             r->meta_kinds.resize(n); r->meta_tx.resize(n); r->meta_lsn.resize(n); r->meta_ct.resize(n); r->selection.resize(r->rows_out);
             CK(cudaMemcpyAsync(r->meta_kinds.data(), B + o_kind, n, cudaMemcpyDeviceToHost, s)); CK(cudaMemcpyAsync(r->meta_tx.data(), B + o_tx, n * 4, cudaMemcpyDeviceToHost, s));
             CK(cudaMemcpyAsync(r->meta_lsn.data(), B + o_lsn, n * 8, cudaMemcpyDeviceToHost, s)); CK(cudaMemcpyAsync(r->meta_ct.data(), B + o_ct, n * 8, cudaMemcpyDeviceToHost, s));
@@ -1701,22 +1672,18 @@ int tfgpu_parse_debezium(tfgpu_engine* e, int plan_id, const char* opts_json, co
         r->consumed = len;
         *out = r.release();
         return TF_OK;
-    } catch (const tfplan::FatalError& f) { return fail(e, f.code, f.what()); }
-    catch (const CudaError& c) { return cuda_fail(e, c); }
-    catch (const std::bad_alloc&) { return fail(e, TF_E_RETRY_OOM, "host allocation failed"); }
-    catch (const std::exception& x) { return fail(e, TF_E_FATAL_CONFIG, x.what()); }
+    });
 }
 
 // debug / profiling aid: cycles thread 0 of every k_lz4_frames CTA spent per phase since enabling (stage, match, parse, scan, emit)
 int tfgpu_debug_lz4_phases(tfgpu_engine* e, int enable, uint64_t out[8]) {
     if (!e) return TF_E_FATAL_ARG;
-    try {
-        CK(cudaSetDevice(e->device));
+    return on_device(e, [&] {
         if (enable && !e->lz_phases) { CK(cudaMalloc(&e->lz_phases, 64)); CK(cudaMemset(e->lz_phases, 0, 64)); }
         if (out && e->lz_phases) { CK(cudaStreamSynchronize(e->stream)); CK(cudaMemcpy(out, e->lz_phases, 64, cudaMemcpyDeviceToHost)); CK(cudaMemset(e->lz_phases, 0, 64)); }
         if (!enable && e->lz_phases) { CK(cudaFree(e->lz_phases)); e->lz_phases = nullptr; }
         return TF_OK;
-    } catch (const CudaError& c) { return cuda_fail(e, c); }
+    });
 }
 
 const uint32_t* tfgpu_result_dbz_msg_sizes(const tfgpu_result* r) { return (r && !r->msg_sizes.empty()) ? r->msg_sizes.data() : nullptr; }
@@ -1741,37 +1708,6 @@ const uint32_t* tfgpu_result_part_ids(const tfgpu_result* r) { return (r && !r->
 const uint32_t* tfgpu_result_key_sizes(const tfgpu_result* r) { return (r && !r->key_sizes.empty()) ? r->key_sizes.data() : nullptr; }
 const uint32_t* tfgpu_result_row_sizes(const tfgpu_result* r) { return (r && !r->row_sizes.empty()) ? r->row_sizes.data() : nullptr; }
 
-// queue JSON serializer batching (pkg/serializer/queue/json_batcher.go:13-66): host only, no device needed
-int tfgpu_queue_debezium_batches(const uint32_t* value_sizes, uint64_t n, uint64_t max_message_size, uint64_t* starts, uint64_t cap, uint64_t* n_msgs) {
-    if ((!value_sizes && n) || !starts || !n_msgs) return TF_E_FATAL_ARG;
-    uint64_t k = 0, cur = 0;
-    for (uint64_t i = 0; i < n; i++) {
-        // expandArrIfNeeded :76-86: a new message for the first value and whenever len(last) + 1 + len(new) > maxMessageSize;
-        // without a limit every value stays its own message (MergeBack :53-65)
-        if (i == 0 || !max_message_size || cur + 1 + value_sizes[i] > max_message_size) { if (k >= cap) return TF_E_FATAL_ARG; starts[k++] = i; cur = 0; }
-        cur += value_sizes[i];
-    }
-    if (k >= cap) return TF_E_FATAL_ARG;
-    starts[k] = n; *n_msgs = k;
-    return TF_OK;
-}
-int tfgpu_queue_json_batches(const uint32_t* row_sizes, uint64_t n, uint64_t max_message_size, uint64_t max_change_items, uint64_t* starts, uint64_t cap, uint64_t* n_msgs) {
-    if ((!row_sizes && n) || !starts || !n_msgs) return TF_E_FATAL_ARG;
-    uint64_t k = 0, start = 0, sum = 0;
-    auto emit = [&](uint64_t s) -> bool { if (k >= cap) return false; starts[k++] = s; return true; };
-    for (uint64_t i = 0; i < n; i++) {
-        const uint64_t count = i - start + 1;
-        const bool viol = (max_message_size && sum + (count - 1) + row_sizes[i] > max_message_size) || (max_change_items && count > max_change_items);
-        if (!viol) { sum += row_sizes[i]; continue; }
-        if (!emit(start)) return TF_E_FATAL_ARG;
-        if (i == start) { start = i + 1; sum = 0; }        // a single item over the size limit goes out alone
-        else { start = i; sum = row_sizes[i]; }
-    }
-    if (start != n && !emit(start)) return TF_E_FATAL_ARG;
-    if (k >= cap) return TF_E_FATAL_ARG;
-    starts[k] = n; *n_msgs = k;
-    return TF_OK;
-}
 void tfgpu_result_release(tfgpu_result* r) {
     if (!r) return;
     if (r->bytes && r->bytes_pinned) cudaFreeHost(r->bytes);   // otherwise the engine's landing buffer
