@@ -2,6 +2,7 @@
 // phase by phase over all "threads", so that parse rules (segment size, probing stride, continuation merging)
 // can be evaluated for compression ratio and validated against a decoder before they are written as a kernel.
 // Development tool, not product code:  g++ -O2 -o /tmp/lz4_model scripts/lz4_model.cpp -ldl && /tmp/lz4_model block.bin
+// (block.bin: the bench.py headline block from scripts/headline_block.py; key=value arguments override the rules below)
 #include <algorithm>
 #include <cstdint>
 #include <cstdio>
@@ -12,11 +13,13 @@
 #include <string>
 #include <vector>
 
+// The defaults are the rules k_lz4_frames runs with.
 struct Cfg {
-    uint32_t F = 30720, SEG = 60, ROUND = 2048, HASH_BITS = 12;
+    uint32_t F = 15360, SEG = 60, ROUND = 1024, HASH_BITS = 11;
     int stride = 2;          // probe every stride-th position (inserts happen at every position)
     bool second_probe = true, period8 = true, merge = true, backext = true;
-    int winner = 2; bool near_first = false; int ins_stride = 1; bool twoslot = false; bool recent_first = false;         // 0 lowest position wins an insert race, 1 highest, 2 random
+    int winner = 3; bool near_first = true; int ins_stride = 1; bool twoslot = false; bool recent_first = false;         // 0 lowest position wins an insert race, 1 highest, 2 random, 3 as in the kernel
+    bool race = false, wmatch = false;
 };
 
 struct Seq { uint32_t p, ml, off; };
@@ -37,13 +40,45 @@ static std::vector<uint8_t> compress_frame(const uint8_t* d, uint32_t len, const
             const uint32_t h = rd32(d, p) * 2654435761u;
             idx[p - r0] = h >> (32 - c.HASH_BITS); tag[p - r0] = (h << c.HASH_BITS) & 0xffff0000u;
         }
+        if (c.race) {
+            // one barrier per round: every warp (32 threads x 4 positions) probes and then inserts, and the warps of a round run in any
+            // order, so a probe sees the inserts of the warps of this round that ran before it (accepted when they lie behind it)
+            const uint32_t WP = 128, nw = (r1 - r0 + WP - 1) / WP;
+            std::vector<uint32_t> worder(nw);
+            for (uint32_t i = 0; i < nw; i++) worder[i] = i;
+            std::shuffle(worder.begin(), worder.end(), rng);
+            for (uint32_t w : worder) {
+                const uint32_t w0 = r0 + w * WP, w1 = std::min(r1, w0 + WP);
+                for (uint32_t p = w0; p < w1; p++) {
+                    if (p % c.stride || p + 12 > len) continue;
+                    if ((p & ~3u) >= 8) {
+                        if (rd32(d, p) == rd32(d, p - 4)) { cand[p] = p - 4; continue; }
+                        if (rd32(d, p) == rd32(d, p - 8)) { cand[p] = p - 8; continue; }
+                    }
+                    const uint32_t e = table[idx[p - r0]];
+                    if (e != 0xffffffffu && (e & 0xffff0000u) == tag[p - r0] && (e & 0xffffu) < p) cand[p] = e & 0xffffu;
+                    if (c.wmatch && cand[p] == 0xffffffffu)      // __match_any_sync: the nearest earlier lane of the warp with the same 4 bytes at the same offset mod 4
+                        for (uint32_t q = p; q >= w0 + 4;) { q -= 4; if (rd32(d, q) == rd32(d, p)) { cand[p] = q; break; } }
+                }
+                std::vector<uint32_t> ord(w1 - w0);
+                for (uint32_t i = 0; i < ord.size(); i++) ord[i] = w0 + i;
+                std::shuffle(ord.begin(), ord.end(), rng);
+                for (uint32_t p : ord) {
+                    if (p + 4 > len || p % c.ins_stride) continue;
+                    uint32_t& e = table[idx[p - r0]];
+                    // winner 0 here: an insert of this round replaces an entry of an earlier round or one of this round behind it (atomicMax)
+                    if (c.winner != 0 || e == 0xffffffffu || (e & 0xffffu) < r0 || (e & 0xffffu) > p) e = tag[p - r0] | p;
+                }
+            }
+            continue;
+        }
         // first probe: the table as it was before this round
         for (uint32_t p = r0; p < r1; p++) {
             if (p % c.stride || p + 12 > len) continue;
             const uint32_t e = table[idx[p - r0]];
-            if (c.near_first) {
-                if (p >= 4 && rd32(d, p) == rd32(d, p - 4)) cand[p] = p - 4;
-                else if (p >= 8 && rd32(d, p) == rd32(d, p - 8)) cand[p] = p - 8;
+            if (c.near_first && (p & ~3u) >= 8) {     // the kernel tests a thread's positions 4 / 8 back from its third word on
+                if (rd32(d, p) == rd32(d, p - 4)) cand[p] = p - 4;
+                else if (rd32(d, p) == rd32(d, p - 8)) cand[p] = p - 8;
             }
             if (cand[p] == 0xffffffffu && e != 0xffffffffu && (e & 0xffff0000u) == tag[p - r0]) cand[p] = e & 0xffffu;
             if (cand[p] == 0xffffffffu && c.period8 && p >= 8 && rd32(d, p) == rd32(d, p - 8)) cand[p] = p - 8;
@@ -53,6 +88,17 @@ static std::vector<uint8_t> compress_frame(const uint8_t* d, uint32_t len, const
         for (uint32_t i = 0; i < order.size(); i++) order[i] = r0 + i;
         if (c.winner == 0) std::reverse(order.begin(), order.end());
         else if (c.winner == 2) std::shuffle(order.begin(), order.end(), rng);
+        else if (c.winner == 3) {
+            // the kernel: warps in any order; a warp stores its lanes' 4th, 3rd, 2nd, 1st positions. Which lane wins a store conflict
+            // is undefined; the lowest lane winning reproduces the kernel's ratio on the bench.py block (1.687 here, 1.693 on the H100)
+            std::vector<uint32_t> ws;
+            for (uint32_t w0 = r0; w0 < r1; w0 += 128) ws.push_back(w0);
+            std::shuffle(ws.begin(), ws.end(), rng);
+            order.clear();
+            for (uint32_t w0 : ws)
+                for (int k = 3; k >= 0; k--)
+                    for (int l = 31; l >= 0; l--) if (w0 + 4 * l + k < r1) order.push_back(w0 + 4 * l + k);
+        }
         for (uint32_t p : order) if (p + 4 <= len && p % c.ins_stride == 0) table[idx[p - r0]] = tag[p - r0] | p;
         if (c.second_probe)
             for (uint32_t p = r0; p < r1; p++) {
@@ -229,6 +275,7 @@ int main(int argc, char** argv) {
         if (k == "F") c.F = v; else if (k == "SEG") c.SEG = v; else if (k == "ROUND") c.ROUND = v; else if (k == "HB") c.HASH_BITS = v;
         else if (k == "stride") c.stride = v; else if (k == "probe2") c.second_probe = v; else if (k == "p8") c.period8 = v;
         else if (k == "merge") c.merge = v; else if (k == "back") c.backext = v; else if (k == "winner") c.winner = v; else if (k == "step") step = v; else if (k == "near") c.near_first = v; else if (k == "ins") c.ins_stride = v; else if (k == "two") c.twoslot = v; else if (k == "recent") c.recent_first = v;
+        else if (k == "race") c.race = v; else if (k == "wmatch") c.wmatch = v;
     }
     typedef int (*comp_t)(const char*, char*, int, int);
     comp_t stock = nullptr;

@@ -3,15 +3,17 @@
 //
 // GPU-native LZ4 (not a port of any CPU compressor): one CTA per frame, the frame lives in shared memory and
 // every phase is data-parallel:
-//   P1  stage the frame in shared memory (16-byte coalesced loads)
+//   P1  stage the frame in shared memory (16-byte coalesced loads, all of a thread's loads in flight at once)
 //   P2  match finding in rounds of 4 x LZ_THREADS positions (4 consecutive per thread: two shared-memory words give the four
 //       4-byte sequences). Every position is inserted into a 2^LZ_HASH_BITS-entry hash table (tag16 | position); every EVEN
 //       position gets a candidate: the same sequence 4 or 8 bytes back (runs of fixed-width values: the nearest
 //       candidate gives the longest match), else the table entry of an earlier round, else (after this round's
-//       inserts) an entry of this round. Result: one u16 candidate per even position + a bitmap.
+//       inserts) an entry of this round. Result: one u16 candidate per even position + two warp ballots per round.
+//       This phase is bound by instruction issue: rounds that lie wholly inside the frame run without bounds tests.
 //   P3  greedy parse, one thread per 60-byte segment (15 words: an odd stride keeps the segment walkers on
 //       different banks). A match found at an even position is extended backwards; matches are cut at the
-//       segment end. Descriptors (offset | length | start) overwrite the segment's candidate slots.
+//       segment end. Descriptors (offset | length | start) overwrite the segment's candidate slots. The walkers
+//       wait on shared memory, so comparisons go 8 bytes forward / 4 bytes backward per round trip.
 //   P3b continuation: a match that was cut at a segment end is carried on by the next segments: each tests how
 //       far the cut match's offset still holds from its first byte (the offset travels over fully matched
 //       segments by a segmented scan); what holds is merged into the running match, so a long match costs one
@@ -78,25 +80,47 @@ __device__ __forceinline__ uint32_t ext_bytes(uint32_t x) { return x < 15 ? 0u :
 __device__ __forceinline__ uint8_t* put_ext(uint8_t* o, uint32_t x) {   // x >= 15
     x -= 15; while (x >= 255) { *o++ = 255; x -= 255; } *o++ = (uint8_t)x; return o;
 }
-// literal copy inside shared memory: frame bytes [src, src + n) -> image bytes at dst (aligned words once dst is aligned)
-__device__ __forceinline__ void copy_lit(uint8_t* dst, const uint32_t* dw, uint32_t src, uint32_t n) {
-    const uint8_t* data = (const uint8_t*)dw;
-    while (n && ((uint32_t)(uintptr_t)dst & 3)) { *dst++ = data[src]; src++; n--; }
-    for (; n >= 4; n -= 4, dst += 4, src += 4) *(uint32_t*)dst = ld32u(dw, src);
-    while (n) { *dst++ = data[src]; src++; n--; }
+__device__ __forceinline__ void put_bytes3(uint8_t* dst, uint32_t x, uint32_t n) {     // the low n (< 4) bytes of x
+#pragma unroll
+    for (uint32_t k = 0; k < 3; k++) if (k < n) dst[k] = (uint8_t)(x >> (8 * k));
 }
-// common prefix of frame bytes at c and p, at most maxl (> 0)
+// literal copy inside shared memory: frame bytes [src, src + n) -> image bytes at dst (aligned words once dst is aligned). Every
+// shared-memory load is a word, and the loads of a step come ahead of its stores: one round trip per 8 bytes and one per ragged end.
+__device__ __forceinline__ void copy_lit(uint8_t* dst, const uint32_t* dw, uint32_t src, uint32_t n) {
+    const uint32_t h = min(n, (0u - (uint32_t)(uintptr_t)dst) & 3u);
+    if (h) { put_bytes3(dst, ld32u(dw, src), h); dst += h; src += h; n -= h; }
+    for (; n >= 8; n -= 8, dst += 8, src += 8) {
+        const uint32_t x = ld32u(dw, src), y = ld32u(dw, src + 4);
+        *(uint32_t*)dst = x; *(uint32_t*)(dst + 4) = y;
+    }
+    if (n >= 4) { *(uint32_t*)dst = ld32u(dw, src); n -= 4; dst += 4; src += 4; }
+    if (n) put_bytes3(dst, ld32u(dw, src), n);
+}
+// common prefix of frame bytes at c and p, at most maxl (> 0). 8 bytes per step: the loads of a step are independent, so a long
+// match waits on half as many shared-memory round trips (the reads run at most 12 bytes past p + maxl, into the guard words)
 __device__ __forceinline__ uint32_t lz_match_len(const uint32_t* dw, uint32_t c, uint32_t p, uint32_t maxl) {
     uint32_t ic = c >> 2, ip = p >> 2; const uint32_t sc = (c & 3) * 8, sp = (p & 3) * 8;
     uint32_t wc0 = dw[ic], wp0 = dw[ip], ml = 0;
     for (;;) {
-        const uint32_t wc1 = dw[++ic], wp1 = dw[++ip];
-        const uint32_t x = __funnelshift_r(wc0, wc1, sc) ^ __funnelshift_r(wp0, wp1, sp);
-        if (x) { ml += (uint32_t)(__ffs((int)x) - 1) >> 3; break; }
-        ml += 4; if (ml >= maxl) break;
-        wc0 = wc1; wp0 = wp1;
+        const uint32_t wc1 = dw[ic + 1], wp1 = dw[ip + 1], wc2 = dw[ic + 2], wp2 = dw[ip + 2];
+        const uint32_t x0 = __funnelshift_r(wc0, wc1, sc) ^ __funnelshift_r(wp0, wp1, sp);
+        const uint32_t x1 = __funnelshift_r(wc1, wc2, sc) ^ __funnelshift_r(wp1, wp2, sp);
+        if (x0 | x1) { ml += x0 ? (uint32_t)(__ffs((int)x0) - 1) >> 3 : 4u + ((uint32_t)(__ffs((int)x1) - 1) >> 3); break; }
+        ml += 8; if (ml >= maxl) break;
+        ic += 2; ip += 2; wc0 = wc2; wp0 = wp2;
     }
     return ml < maxl ? ml : maxl;
+}
+// common suffix of the frame bytes in front of c and p, at most maxb: how far a match found at p extends backwards
+__device__ __forceinline__ uint32_t lz_back_len(const uint32_t* dw, uint32_t c, uint32_t p, uint32_t maxb) {
+    uint32_t n = 0;
+    while (n < maxb) {      // 4 bytes per step, the last one highest; maxb <= c, so a read starts at most 3 bytes in front of the frame (zero guards)
+        const int32_t qc = (int32_t)(c - n) - 4, qp = (int32_t)(p - n) - 4;
+        const uint32_t x = __funnelshift_r(dw[qc >> 2], dw[(qc >> 2) + 1], (qc & 3) * 8) ^ __funnelshift_r(dw[qp >> 2], dw[(qp >> 2) + 1], (qp & 3) * 8);
+        if (x) { n += (uint32_t)__clz((int)x) >> 3; break; }
+        n += 4;
+    }
+    return n < maxb ? n : maxb;
 }
 
 // Decoupled look-back (warp 0 only): the exclusive prefix of the sizes of frames [0, f). Cells hold AGG | own size or INCL | inclusive prefix.
@@ -131,15 +155,55 @@ __device__ __forceinline__ unsigned long long lz_lookback(const Lz4Args& a, uint
 }
 
 #ifdef TF_KERNELS_LZ4
+// One match-finding round (P2): thread wi takes positions 4 wi .. 4 wi + 3. FULL: every position of the round is inside the frame
+// (all rounds but a short last one), so the round runs without the per-thread bounds test and the branches around it.
+template <bool FULL>
+__device__ __forceinline__ void lz_match_round(const uint32_t* dw, uint32_t* table, uint32_t* cand_w, uint32_t* bm, uint32_t wi, uint32_t lane, uint32_t len) {
+    const uint32_t p0 = wi * 4;
+    const bool active = FULL || p0 < len;
+    uint32_t i0 = 0, i1 = 0, i2 = 0, i3 = 0, e0 = 0, e1 = 0, e2 = 0, e3 = 0, c0 = LZ_NONE, c2 = LZ_NONE, t0 = 0, t2 = 0;
+    if (active) {
+        const uint32_t wm2 = dw[(int)wi - 2], wm1 = dw[(int)wi - 1], w0 = dw[wi], w1 = dw[wi + 1];
+        const uint32_t s1 = __funnelshift_r(w0, w1, 8), s2 = __funnelshift_r(w0, w1, 16), s3 = __funnelshift_r(w0, w1, 24);
+        const uint32_t h0 = w0 * 2654435761u, h1 = s1 * 2654435761u, h2 = s2 * 2654435761u, h3 = s3 * 2654435761u;
+        i0 = h0 >> (32 - LZ_HASH_BITS); i1 = h1 >> (32 - LZ_HASH_BITS); i2 = h2 >> (32 - LZ_HASH_BITS); i3 = h3 >> (32 - LZ_HASH_BITS);
+        e0 = ((h0 << LZ_HASH_BITS) & 0xffff0000u) | p0; e1 = ((h1 << LZ_HASH_BITS) & 0xffff0000u) | (p0 + 1);
+        e2 = ((h2 << LZ_HASH_BITS) & 0xffff0000u) | (p0 + 2); e3 = ((h3 << LZ_HASH_BITS) & 0xffff0000u) | (p0 + 3);
+        // the same 4 bytes 4 or 8 back: a run of a fixed-width value (from the third word on; the first two read the zero guards)
+        const uint32_t a2 = __funnelshift_r(wm1, w0, 16), b2 = __funnelshift_r(wm2, wm1, 16);
+        c0 = w0 == wm1 ? p0 - 4 : (w0 == wm2 ? p0 - 8 : LZ_NONE);
+        c2 = s2 == a2 ? p0 - 2 : (s2 == b2 ? p0 - 6 : LZ_NONE);
+        if (p0 < 8) c0 = c2 = LZ_NONE;
+        t0 = table[i0]; t2 = table[i2];
+    }
+    __syncthreads();
+    if (active) {
+        table[i3] = e3; table[i2] = e2; table[i1] = e1; table[i0] = e0;
+        if (c0 == LZ_NONE && ((t0 ^ e0) >> 16) == 0) c0 = t0 & 0xffffu;      // an entry of an earlier round: position < p0
+        if (c2 == LZ_NONE && ((t2 ^ e2) >> 16) == 0) c2 = t2 & 0xffffu;
+    }
+    __syncthreads();
+    if (active) {   // second probe: sees this round's inserts, recovers repeats whose first occurrence is in this round
+        if (c0 == LZ_NONE) { const uint32_t t = table[i0]; if (((t ^ e0) >> 16) == 0 && (t & 0xffffu) < p0) c0 = t & 0xffffu; }
+        if (c2 == LZ_NONE) { const uint32_t t = table[i2]; if (((t ^ e2) >> 16) == 0 && (t & 0xffffu) < p0 + 2) c2 = t & 0xffffu; }
+        cand_w[wi] = (c0 & 0xffffu) | (c2 << 16);
+    }
+    const uint32_t b0 = __ballot_sync(0xffffffffu, c0 != LZ_NONE), b2 = __ballot_sync(0xffffffffu, c2 != LZ_NONE);
+    if (lane == 0) { bm[2 * (wi >> 5)] = b0; bm[2 * (wi >> 5) + 1] = b2; }
+}
+// bit j of x (< 2^16) -> bit 2 j
+__device__ __forceinline__ uint32_t lz_spread(uint32_t x) {
+    x = (x | (x << 8)) & 0x00ff00ffu; x = (x | (x << 4)) & 0x0f0f0f0fu; x = (x | (x << 2)) & 0x33333333u; return (x | (x << 1)) & 0x55555555u;
+}
+
 __global__ void __launch_bounds__(LZ_THREADS, LZ_CTAS_PER_SM) k_lz4_frames(Lz4Args a) {
     extern __shared__ __align__(16) uint8_t smem[];
     const uint32_t F = a.frame_bytes;
     const LzSmem L = lz_smem(F);
     uint32_t* dw = (uint32_t*)(smem + L.data);                   // the frame; dw[-2], dw[-1] and 4 words behind it are zero guards
-    const uint8_t* data = smem + L.data;
     uint16_t* cand = (uint16_t*)(smem + L.cand);                // candidate of even position p at cand[p >> 1]; later: sequence descriptors
     uint32_t* cand_w = (uint32_t*)(smem + L.cand);
-    uint32_t* bm = (uint32_t*)(smem + L.bitmap);                // bit i: position 2 i has a candidate
+    uint32_t* bm = (uint32_t*)(smem + L.bitmap);                // per warp and round the ballots [p0 has a candidate][p0 + 2 has one]: bit i of word 2 j (+ 1) is P2 thread 32 j + i
     uint32_t* table = (uint32_t*)(smem + L.table);
     uint8_t* stg = smem + L.stg;                                // [0x82][u32 size + 9][u32 raw size][LZ4 block]
     __shared__ uint32_t s_frame;
@@ -203,7 +267,12 @@ __global__ void __launch_bounds__(LZ_THREADS, LZ_CTAS_PER_SM) k_lz4_frames(Lz4Ar
             const int4* g = (const int4*)(a.raw + pos0);
             const uint32_t nv = (len + 15) >> 4;
             int4* d4 = (int4*)(smem + L.data);
-            for (uint32_t i = tid; i < nv + 1; i += LZ_THREADS) d4[i] = i < nv ? __ldg(g + i) : make_int4(0, 0, 0, 0);
+            constexpr uint32_t NLD = (LZ_MAX_FRAME / 16 + LZ_THREADS) / LZ_THREADS;     // the frame and a zero guard: all loads in flight at once
+            int4 v[NLD];
+#pragma unroll
+            for (uint32_t k = 0; k < NLD; k++) { const uint32_t i = tid + k * LZ_THREADS; v[k] = i < nv ? __ldg(g + i) : make_int4(0, 0, 0, 0); }
+#pragma unroll
+            for (uint32_t k = 0; k < NLD; k++) { const uint32_t i = tid + k * LZ_THREADS; if (i < nv + 1) d4[i] = v[k]; }
             int4* t4 = (int4*)table;
             for (uint32_t i = tid; i < (1u << LZ_HASH_BITS) / 4; i += LZ_THREADS) t4[i] = make_int4(0, 0, 0, 0);
             if (tid < 4) ((uint32_t*)smem)[tid] = 0;
@@ -213,43 +282,9 @@ __global__ void __launch_bounds__(LZ_THREADS, LZ_CTAS_PER_SM) k_lz4_frames(Lz4Ar
         LZ_PHASE(0);
         // ---- P2: match finding
         const uint32_t nrounds = (len + LZ_ROUND - 1) / LZ_ROUND;
-        for (uint32_t rd = 0; rd < nrounds; rd++) {
-            const uint32_t wi = rd * LZ_THREADS + tid, p0 = wi * 4;
-            const bool active = p0 < len;
-            uint32_t i0 = 0, i1 = 0, i2 = 0, i3 = 0, e0 = 0, e1 = 0, e2 = 0, e3 = 0, c0 = LZ_NONE, c2 = LZ_NONE, t0 = 0, t2 = 0;
-            if (active) {
-                const uint32_t wm2 = dw[(int)wi - 2], wm1 = dw[(int)wi - 1], w0 = dw[wi], w1 = dw[wi + 1];
-                const uint32_t s1 = __funnelshift_r(w0, w1, 8), s2 = __funnelshift_r(w0, w1, 16), s3 = __funnelshift_r(w0, w1, 24);
-                const uint32_t h0 = w0 * 2654435761u, h1 = s1 * 2654435761u, h2 = s2 * 2654435761u, h3 = s3 * 2654435761u;
-                i0 = h0 >> (32 - LZ_HASH_BITS); i1 = h1 >> (32 - LZ_HASH_BITS); i2 = h2 >> (32 - LZ_HASH_BITS); i3 = h3 >> (32 - LZ_HASH_BITS);
-                e0 = ((h0 << LZ_HASH_BITS) & 0xffff0000u) | p0; e1 = ((h1 << LZ_HASH_BITS) & 0xffff0000u) | (p0 + 1);
-                e2 = ((h2 << LZ_HASH_BITS) & 0xffff0000u) | (p0 + 2); e3 = ((h3 << LZ_HASH_BITS) & 0xffff0000u) | (p0 + 3);
-                if (p0 >= 8) {      // the same 4 bytes 4 or 8 back: a run of a fixed-width value
-                    const uint32_t a2 = __funnelshift_r(wm1, w0, 16), b2 = __funnelshift_r(wm2, wm1, 16);
-                    c0 = w0 == wm1 ? p0 - 4 : (w0 == wm2 ? p0 - 8 : LZ_NONE);
-                    c2 = s2 == a2 ? p0 - 2 : (s2 == b2 ? p0 - 6 : LZ_NONE);
-                }
-                t0 = table[i0]; t2 = table[i2];
-            }
-            __syncthreads();
-            if (active) {
-                table[i3] = e3; table[i2] = e2; table[i1] = e1; table[i0] = e0;
-                if (c0 == LZ_NONE && ((t0 ^ e0) >> 16) == 0) c0 = t0 & 0xffffu;      // an entry of an earlier round: position < p0
-                if (c2 == LZ_NONE && ((t2 ^ e2) >> 16) == 0) c2 = t2 & 0xffffu;
-            }
-            __syncthreads();
-            uint32_t v = 0;
-            if (active) {   // second probe: sees this round's inserts, recovers repeats whose first occurrence is in this round
-                if (c0 == LZ_NONE) { const uint32_t t = table[i0]; if (((t ^ e0) >> 16) == 0 && (t & 0xffffu) < p0) c0 = t & 0xffffu; }
-                if (c2 == LZ_NONE) { const uint32_t t = table[i2]; if (((t ^ e2) >> 16) == 0 && (t & 0xffffu) < p0 + 2) c2 = t & 0xffffu; }
-                cand_w[wi] = (c0 & 0xffffu) | (c2 << 16);
-                v = (c0 != LZ_NONE ? 1u : 0u) | (c2 != LZ_NONE ? 2u : 0u);
-            }
-            // 2 bits per lane -> the warp's 64 bitmap bits
-            const uint32_t x = v << (2 * (lane & 15));
-            const uint32_t lo = __reduce_or_sync(0xffffffffu, lane < 16 ? x : 0u), hi = __reduce_or_sync(0xffffffffu, lane < 16 ? 0u : x);
-            if (lane == 0) { bm[wi >> 4] = lo; bm[(wi >> 4) + 1] = hi; }
-        }
+        const uint32_t nfull = len / LZ_ROUND;
+        for (uint32_t rd = 0; rd < nfull; rd++) lz_match_round<true>(dw, table, cand_w, bm, rd * LZ_THREADS + tid, lane, len);
+        if (nfull < nrounds) lz_match_round<false>(dw, table, cand_w, bm, nfull * LZ_THREADS + tid, lane, len);
         if (tid == 0) { bm[((nrounds * LZ_THREADS) >> 4)] = 0; bm[((nrounds * LZ_THREADS) >> 4) + 1] = 0; }
         __syncthreads();
         if (tid == 0) bm[0] &= ~1u;        // position 0 has nothing before it
@@ -266,8 +301,9 @@ __global__ void __launch_bounds__(LZ_THREADS, LZ_CTAS_PER_SM) k_lz4_frames(Lz4Ar
         if (tid < nseg) {
             sb = sa + LZ_SEG < len ? sa + LZ_SEG : len;
             slimit = sb < lim5 ? sb : lim5;
-            const uint32_t bi = tid * (LZ_SEG / 2);
-            const uint32_t m = __funnelshift_r(bm[bi >> 5], bm[(bi >> 5) + 1], bi & 31) & 0x3fffffffu;
+            const uint32_t k = tid * (LZ_SEG / 4), bw = 2 * (k >> 5);      // the segment's first P2 thread, its ballot pair
+            const uint32_t m0 = __funnelshift_r(bm[bw], bm[bw + 2], k & 31) & 0x7fffu, m2 = __funnelshift_r(bm[bw + 1], bm[bw + 3], k & 31) & 0x7fffu;
+            const uint32_t m = lz_spread(m0) | (lz_spread(m2) << 1);       // bit j: position sa + 2 j has a candidate
             uint32_t cur = 0, anchor = sa;
             for (;;) {
                 const uint32_t cb = (cur + 1) >> 1;
@@ -280,7 +316,8 @@ __global__ void __launch_bounds__(LZ_THREADS, LZ_CTAS_PER_SM) k_lz4_frames(Lz4Ar
                 uint32_t c = cand[p >> 1];
                 uint32_t ml = lz_match_len(dw, c, p, slimit - p);
                 if (ml < 4) { cur = 2 * r + 1; continue; }              // the tag agreed but the bytes do not: not a match
-                while (p > anchor && c > 0 && data[p - 1] == data[c - 1]) { p--; c--; ml++; }
+                const uint32_t nb = lz_back_len(dw, c, p, min(p - anchor, c));
+                p -= nb; c -= nb; ml += nb;
                 desc[nseq++] = ((p - c) << 16) | (ml << 8) | (p - sa);
                 d_last = p - c;
                 anchor = p + ml; cur = anchor - sa;
@@ -310,12 +347,12 @@ __global__ void __launch_bounds__(LZ_THREADS, LZ_CTAS_PER_SM) k_lz4_frames(Lz4Ar
                 const uint32_t maxn = slimit - sa;
                 const uint32_t q = sa - D; uint32_t iq = q >> 2; const uint32_t sq = (q & 3) * 8;
                 uint32_t wq0 = dw[iq]; const uint32_t* pw = dw + tid * (LZ_SEG / 4);
-                for (;;) {
-                    const uint32_t wq1 = dw[++iq];
-                    const uint32_t x = __funnelshift_r(wq0, wq1, sq) ^ pw[n >> 2];
-                    if (x) { n += (uint32_t)(__ffs((int)x) - 1) >> 3; break; }
-                    n += 4; if (n >= maxn) break;
-                    wq0 = wq1;
+                for (;;) {      // 8 bytes per step, as lz_match_len
+                    const uint32_t wq1 = dw[iq + 1], wq2 = dw[iq + 2];
+                    const uint32_t x0 = __funnelshift_r(wq0, wq1, sq) ^ pw[n >> 2], x1 = __funnelshift_r(wq1, wq2, sq) ^ pw[(n >> 2) + 1];
+                    if (x0 | x1) { n += x0 ? (uint32_t)(__ffs((int)x0) - 1) >> 3 : 4u + ((uint32_t)(__ffs((int)x1) - 1) >> 3); break; }
+                    n += 8; if (n >= maxn) break;
+                    iq += 2; wq0 = wq2;
                 }
                 if (n > maxn) n = maxn;
             }
