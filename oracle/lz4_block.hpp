@@ -60,27 +60,39 @@ inline size_t lz4_compress(const uint8_t* src, size_t n, uint8_t* dst) {
     return (size_t)(op - dst);
 }
 
-// Safe decoder; returns decoded size or (size_t)-1 on malformed input.
-inline size_t lz4_decompress(const uint8_t* src, size_t n, uint8_t* dst, size_t cap) {
+// Strict decoder of one block of exactly rs raw bytes; returns rs, or (size_t)-1 when the block is malformed or breaks a
+// rule of the block format that decoders copying in wide chunks rely on (lz4_Block_format.md, "End of block conditions"):
+//   - the last sequence holds literals only (the block ends right behind a literal run, never behind a match);
+//   - no match starts within the last 12 bytes (start <= rs - 12), so a block of fewer than 13 bytes has no match;
+//   - no match reaches into the last 5 bytes (end <= rs - 5);
+//   - offsets are in [1, bytes decoded so far]; length extensions and offsets are complete;
+//   - the input is used up exactly when rs bytes have been decoded.
+inline size_t lz4_decompress(const uint8_t* src, size_t n, uint8_t* dst, size_t rs) {
+    const size_t MFLIMIT = 12, LASTLIT = 5;
+    const size_t bad = (size_t)-1;
     size_t ip = 0, op = 0;
-    while (ip < n) {
-        uint8_t tok = src[ip++];
+    if (n == 0) return bad;                                        // not even the token of the last sequence
+    for (;;) {
+        const uint8_t tok = src[ip++];
         size_t ll = tok >> 4;
-        if (ll == 15) { uint8_t b; do { if (ip >= n) return (size_t)-1; b = src[ip++]; ll += b; } while (b == 255); }
-        if (ip + ll > n || op + ll > cap) return (size_t)-1;
+        if (ll == 15) { uint8_t b; do { if (ip >= n) return bad; b = src[ip++]; ll += b; } while (b == 255); }
+        if (ll > n - ip || ll > rs - op) return bad;
         std::memcpy(dst + op, src + ip, ll); ip += ll; op += ll;
-        if (ip >= n) break;
-        if (ip + 2 > n) return (size_t)-1;
-        size_t off = src[ip] | (src[ip + 1] << 8); ip += 2;
-        if (off == 0 || off > op) return (size_t)-1;
+        if (ip == n) break;                                       // literal-only last sequence
+        if (op == rs) return bad;                                 // trailing input behind a complete block
+        if (n - ip < 2) return bad;
+        const size_t off = src[ip] | (src[ip + 1] << 8); ip += 2;
+        if (off == 0 || off > op) return bad;
         size_t ml = tok & 15;
-        if (ml == 15) { uint8_t b; do { if (ip >= n) return (size_t)-1; b = src[ip++]; ml += b; } while (b == 255); }
+        if (ml == 15) { uint8_t b; do { if (ip >= n) return bad; b = src[ip++]; ml += b; } while (b == 255); }
         ml += 4;
-        if (op + ml > cap) return (size_t)-1;
+        if (rs < MFLIMIT + 1 || op > rs - MFLIMIT) return bad;    // match starts within the last 12 bytes
+        if (ml > rs - LASTLIT - op) return bad;                   // match reaches into the last 5 bytes
         for (size_t i = 0; i < ml; i++) dst[op + i] = dst[op + i - off];
         op += ml;
+        if (ip == n) return bad;                                  // the block ends behind a match
     }
-    return op;
+    return op == rs ? op : bad;
 }
 
 // Cut `raw` into frames of at most frame_bytes raw bytes and wrap each one.

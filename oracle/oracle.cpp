@@ -560,7 +560,7 @@ void orc_sha256(const uint8_t* msg, uint64_t mlen, uint8_t out[32]) { Sha256 s; 
 void orc_cityhash128(const uint8_t* p, uint64_t n, uint64_t* lo, uint64_t* hi) { city::u128 h = city::hash128(p, n); *lo = h.first; *hi = h.second; }
 uint64_t orc_lz4_bound(uint64_t n) { return lz4_bound(n); }
 uint64_t orc_lz4_compress(const uint8_t* src, uint64_t n, uint8_t* dst) { return lz4_compress(src, n, dst); }
-int64_t orc_lz4_decompress(const uint8_t* src, uint64_t n, uint8_t* dst, uint64_t cap) { size_t r = lz4_decompress(src, n, dst, cap); return r == (size_t)-1 ? -1 : (int64_t)r; }
+int64_t orc_lz4_decompress(const uint8_t* src, uint64_t n, uint8_t* dst, uint64_t rs) { size_t r = lz4_decompress(src, n, dst, rs); return r == (size_t)-1 ? -1 : (int64_t)r; }
 
 int orc_match_value(const orc_val* v, const orc_term* t, int* matched) { bool m = false; int rc = match_value(*v, *t, m); *matched = m; return rc; }
 

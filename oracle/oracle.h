@@ -87,7 +87,8 @@ void orc_sha256(const uint8_t* msg, uint64_t mlen, uint8_t out[32]);
 void orc_cityhash128(const uint8_t* p, uint64_t n, uint64_t* lo, uint64_t* hi);
 uint64_t orc_lz4_bound(uint64_t n);
 uint64_t orc_lz4_compress(const uint8_t* src, uint64_t n, uint8_t* dst);
-int64_t  orc_lz4_decompress(const uint8_t* src, uint64_t n, uint8_t* dst, uint64_t cap);
+/* Strict: decodes a block of exactly rs raw bytes that obeys the LZ4 end-of-block rules (lz4_block.hpp), else -1. */
+int64_t  orc_lz4_decompress(const uint8_t* src, uint64_t n, uint8_t* dst, uint64_t rs);
 /* matchValue: returns 0 ok (*matched set), else TF_ROWERR_* */
 int  orc_match_value(const orc_val* v, const orc_term* t, int* matched);
 
@@ -178,7 +179,7 @@ int orc_queue_json_batches(const uint64_t* len_elements, uint64_t n, uint64_t ma
 /* Measurer middleware: Size.Values = util.DeepSizeof(ColumnValues) per row (pkg/util/sizeof.go:7-110). */
 int orc_measure(const tf_batch* in, uint64_t* per_row, uint64_t* total);
 
-/* Verify + decode a frame stream with the oracle's own LZ4 decoder and CityHash. */
+/* Verify + decode a frame stream with the oracle's own (strict) LZ4 decoder and CityHash. */
 int orc_ch_decode_frames(const uint8_t* wire, uint64_t n, orc_buf* raw, uint64_t* n_frames);
 
 #ifdef __cplusplus

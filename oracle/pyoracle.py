@@ -175,6 +175,7 @@ def lz4_compress(data: bytes) -> bytes:
 
 
 def lz4_decompress(data: bytes, raw_len: int) -> Optional[bytes]:
+    """The block of exactly raw_len bytes, or None when it is malformed or breaks an LZ4 end-of-block rule (lz4_block.hpp)."""
     src = (C.c_uint8 * max(1, len(data))).from_buffer_copy(data or b"\0"); dst = (C.c_uint8 * max(1, raw_len))()
     r = lib().orc_lz4_decompress(src, len(data), dst, raw_len)
     return None if r < 0 else bytes(dst[:r])

@@ -280,7 +280,7 @@ def test_resident_batches_back_to_back(eng, po):
     assert raw == po.push_encode(small, plan, RAW).raw
 
 
-@pytest.mark.parametrize("frame_bytes", [1024, 4096, 12288, 15360])
+@pytest.mark.parametrize("frame_bytes", [1024, 1040, 4096, 12288, 15344, 15360])
 def test_other_frame_sizes(po, frame_bytes):
     e = engine.Engine(0, frame_bytes)
     try:

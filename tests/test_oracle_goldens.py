@@ -173,11 +173,33 @@ def test_sha_hmac_vs_hashlib(po):
             assert po.hmac_hex(key, msg) == hmac.new(key, msg, hashlib.sha256).hexdigest()
 
 
+def lz4_block(seqs, last: bytes) -> bytes:
+    """An LZ4 block written by hand: (literals, offset, match length) sequences, then the literal-only last sequence.
+    Offsets and lengths are written as given, legal or not."""
+    def ext(x):
+        out = b""
+        while x >= 255:
+            out += b"\xff"; x -= 255
+        return out + bytes([x])
+    out = b""
+    for lit, off, ml in seqs:
+        ll, mt = len(lit), ml - 4
+        out += bytes([(min(ll, 15) << 4) | min(mt, 15)]) + (ext(ll - 15) if ll >= 15 else b"") + lit
+        out += struct.pack("<H", off) + (ext(mt - 15) if mt >= 15 else b"")
+    return out + bytes([min(len(last), 15) << 4]) + (ext(len(last) - 15) if len(last) >= 15 else b"") + last
+
+
 def test_lz4_oracle_vs_liblz4_and_pyarrow(po):
     import pyarrow as pa
     lz = C.CDLL("liblz4.so.1")
     rnd = np.random.default_rng(11)
     samples = [b"", b"a", b"abcabcabcabcabcabcabcabc" * 50, bytes(rnd.integers(0, 256, 5000, dtype=np.uint8)), bytes(rnd.integers(0, 4, 70000, dtype=np.uint8)), b"\0" * 100000]
+    # every short length (the end-of-block rules decide everything below ~40 bytes) and long runs at the length-extension steps
+    noise = bytes(rnd.integers(0, 256, 600, dtype=np.uint8))
+    for n in range(41):
+        samples += [b"\0" * n, (b"abcab" * 9)[:n], noise[:n]]
+    for n in (13, 17, 18, 19, 20, 274, 275, 529, 70000):
+        samples += [b"x" * n, noise[:7] + b"y" * n + noise[7:40], noise[:300] + noise[:n % 300] + noise[:9]]
     codec = pa.Codec("lz4_raw")
     for s in samples:
         c = po.lz4_compress(s)
@@ -190,6 +212,44 @@ def test_lz4_oracle_vs_liblz4_and_pyarrow(po):
         cap = lz.LZ4_compressBound(len(s)); buf = C.create_string_buffer(max(1, cap))
         n = lz.LZ4_compress_default(s, buf, len(s), cap)
         assert po.lz4_decompress(buf.raw[:n], len(s)) == s
+
+    # The oracle decoder is strict: hand-built blocks of 32 raw bytes (12 for the short one), each breaking one rule.
+    u = bytes(range(100, 164))                        # no byte repeats: a literal never continues a match by accident
+    ok = {                                            # the limits themselves are legal
+        "match at rs - 12": (lz4_block([(u[:20], 20, 4)], u[20:28]), 32),
+        "match ending at rs - 5": (lz4_block([(u[:8], 8, 19)], u[8:13]), 32),
+        "extended lengths": (lz4_block([(u[:15], 15, 19)], u[15:61]), 80),
+        "12 literals": (lz4_block([], u[:12]), 12),
+        "empty block": (b"\x00", 0),
+    }
+    for what, (blk, rs) in ok.items():
+        got = po.lz4_decompress(blk, rs)
+        assert got is not None and len(got) == rs, what
+        dst = C.create_string_buffer(max(1, rs))
+        assert lz.LZ4_decompress_safe(blk, dst, len(blk), rs) == rs and dst.raw[:rs] == got, what
+    valid = lz4_block([(u[:8], 8, 8)], u[8:24])
+    assert po.lz4_decompress(valid, 32) == u[:8] * 2 + u[8:24]
+    m8 = bytes([(8 << 4) | 15]) + u[:8] + b"\x08\x00"         # a match token whose length extension is cut off
+    bad = {
+        "ends after a match": (lz4_block([(u[:1], 1, 31)], b"")[:-1], 32),     # (so its match also covers the last 5 bytes)
+        "match starts after rs - 12": (lz4_block([(u[:21], 21, 4)], u[21:28]), 32),
+        "match ends after rs - 5": (lz4_block([(u[:8], 8, 20)], u[8:12]), 32),
+        "match in a block of 12 bytes": (lz4_block([(u[:1], 1, 4)], u[1:8]), 12),
+        "offset 0": (lz4_block([(u[:8], 0, 8)], u[8:24]), 32),
+        "offset behind the block start": (lz4_block([(u[:8], 9, 8)], u[8:24]), 32),
+        "truncated literal length": (b"\xf0\xff", 270),
+        "truncated match length": (m8, 32),
+        "truncated offset": (bytes([8 << 4]) + u[:8] + b"\x08", 32),
+        "trailing input": (valid + b"\x00", 32),
+        "decodes short": (valid, 33),
+        "decodes long": (valid, 31),
+        "no token": (b"", 0),
+    }
+    for what, (blk, rs) in bad.items():
+        assert po.lz4_decompress(blk, rs) is None, what
+        # the same block inside a frame with valid header and checksum: the frame walk rejects it too
+        body = bytes([0x82]) + struct.pack("<II", len(blk) + 9, rs) + blk
+        assert po.ch_decode_frames(struct.pack("<QQ", *po.cityhash128(body)) + body) == (None, 0), what
 
 
 def test_native_block_bytes_hand_computed(po):
