@@ -178,6 +178,19 @@ typedef struct tf_rowerr {
 #define TF_WIRE_DEBEZIUM       6  /* tfgpu_emit_debezium only: key message + value message per row  */
 #define TF_WIRE_F_CLOSING_NEWLINE 0x100  /* JSONSerializerConfig.AddClosingNewLine (json.go:15)   */
 #define TF_WIRE_F_ANY_AS_STRING   0x200  /* JSONSerializerConfig.AnyAsString (json_format.go:69-76) */
+/* The S3 sink's OutputEncoding (pkg/providers/s3/sink/writer/writer.go:45-55, uploader.go:29-47): the row text of TF_WIRE_SER_JSON /
+ * TF_WIRE_SER_CSV compressed on the device, as one gzip member (RFC 1952) or one zlib stream (RFC 1950). At most one of the two, and
+ * only on the serializer formats (any other combination is TF_E_FATAL_UNSUPPORTED). tfgpu_result_bytes / _bytes_len give the
+ * container, tfgpu_result_raw_len the length of the text inside it; row sizes, rows, selection, errors and part ids are those of the
+ * same call without the flag. Layout of the container (tfgpu_deflate_stream_* relies on it):
+ *   header      gzip 1f 8b 08 00 00000000 00 ff (no name, MTIME 0, XFL 0, OS 255) | zlib 78 9c: what Go's default writers emit
+ *   chunks      the text cut into 16 KiB chunks, compressed independently (no back-reference crosses a chunk start); every chunk
+ *               starts byte-aligned and ends with a sync-flush marker (an empty non-final stored block: ... 00 00 ff ff)
+ *   final block 03 00 (an empty final fixed-Huffman block)
+ *   trailer     gzip CRC-32 + ISIZE (little-endian) | zlib Adler-32 (big-endian)
+ * The compressed bytes are not those of Go's compress/flate: the text they decode to and the framing above are what is pinned. */
+#define TF_WIRE_F_GZIP            0x400
+#define TF_WIRE_F_ZLIB            0x800
 
 typedef struct tfgpu_engine tfgpu_engine;
 typedef struct tfgpu_result tfgpu_result;
@@ -415,6 +428,24 @@ int tfgpu_queue_json_batches(const uint32_t* json_row_sizes, uint64_t n, uint64_
  * row of every merged message as tfgpu_queue_json_batches does. max_message_size == 0: the reference does not merge (MergeBack). Host only. */
 int tfgpu_queue_debezium_batches(const uint32_t* value_sizes, uint64_t n, uint64_t max_message_size, uint64_t* starts, uint64_t cap, uint64_t* n_msgs);
 void              tfgpu_result_release(tfgpu_result* r);
+
+/* One object out of many pushes (host only): the snapshot writer streams every batch of a file through one gzip / zlib writer, and a
+ * zlib object cannot be a concatenation of streams. A stream joins the results of TF_WIRE_F_GZIP (or TF_WIRE_F_ZLIB) pushes, in
+ * order, into one gzip member (one zlib stream) that decodes to the concatenation of their texts: the header once, every result's
+ * chunks, then the final block and a trailer with the checksums combined (ISIZE = total text length mod 2^32).
+ *   open    container = TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB
+ *   append  one result: its bytes / bytes_len / raw_len (tfgpu_result_bytes, _bytes_len, _raw_len). The first append also writes
+ *           the header. *written = bytes put at out. A result whose header, final block or trailer does not match the container
+ *           (or whose gzip ISIZE is not raw_len mod 2^32) is refused with TF_E_FATAL_ARG, as is out too small (cap); the stream
+ *           is unchanged then.
+ *   close   the final block and the trailer (after the header when nothing was appended): *written bytes at out.
+ * Returns TF_OK or TF_E_FATAL_ARG. */
+typedef struct tfgpu_deflate_stream tfgpu_deflate_stream;
+int  tfgpu_deflate_stream_open(int container, tfgpu_deflate_stream** out);
+int  tfgpu_deflate_stream_append(tfgpu_deflate_stream* s, const uint8_t* bytes, uint64_t len, uint64_t raw_len, uint8_t* out, uint64_t cap,
+                                 uint64_t* written);
+int  tfgpu_deflate_stream_close(tfgpu_deflate_stream* s, uint8_t* out, uint64_t cap, uint64_t* written);
+void tfgpu_deflate_stream_free(tfgpu_deflate_stream* s);
 
 /* Number of kernel launches issued by this engine since creation (bench `gpu_launches`). */
 uint64_t tfgpu_engine_launch_count(const tfgpu_engine* e);

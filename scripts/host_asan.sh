@@ -5,13 +5,13 @@
 set -e
 ROOT=$(cd "$(dirname "$0")/.." && pwd); OUT=${1:-/tmp/tfhost_asan}; mkdir -p "$OUT"
 CSRC="$ROOT/transferia_b200/csrc"
-HOST_TUS=("$CSRC/host_rows.cu" "$CSRC/host_sink.cu" "$CSRC/host_chwire.cu" "$CSRC/host_plan.cu")
-python - "$ROOT" "$OUT" "$CSRC/host_plan.cu" <<'PY'
+HOST_TUS=("$CSRC/host_rows.cu" "$CSRC/host_sink.cu" "$CSRC/host_chwire.cu" "$CSRC/host_plan.cu" "$CSRC/host_deflate.cu")
+python - "$ROOT" "$OUT" "$CSRC/host_plan.cu" "$CSRC/host_deflate.cu" <<'PY'
 import re, sys
-root, out, host_plan = sys.argv[1], sys.argv[2], sys.argv[3]
+root, out, host_defs = sys.argv[1], sys.argv[2], sys.argv[3:]
 hdr = re.sub(r"/\*.*?\*/", "", open(root + "/include/tfgpu.h").read(), flags=re.S)
 protos = re.findall(r"^\s*((?:const\s+)?[\w]+(?:\s*\*)?)\s+(tfgpu_\w+)\s*\(([^;{]*?)\)\s*;", hdr, flags=re.M | re.S)
-real = set(re.findall(r"^int (tfgpu_\w+)\(", open(host_plan).read(), flags=re.M))     # defined by host_plan.cu, compiled below
+real = set(n for f in host_defs for n in re.findall(r"^(?:int|void) (tfgpu_\w+)\(", open(f).read(), flags=re.M))     # defined by host_plan.cu / host_deflate.cu, compiled below
 lines = ['#include "%s/include/tfgpu.h"' % root, 'extern "C" {']
 for ret, name, args in protos:
     if name in real:
@@ -27,6 +27,10 @@ TFGPU_LIB_PATH="$OUT/libtfhost_asan.so" LD_PRELOAD="$(gcc -print-file-name=libas
     ASAN_OPTIONS=detect_leaks=0:halt_on_error=1 UBSAN_OPTIONS=print_stacktrace=1:halt_on_error=1 \
     python -m pytest tests/test_rows.py tests/test_sink_push.py tests/test_ch_wire.py tests/test_host_cpu.py tests/test_regex_replace.py -q -m "not gpu" -p no:cacheprovider \
     -k "not exports and not sm90a and not no_cpu_fallback and not gloo and not bench_reference and not c_example"
+# the deflate stream helper (host_deflate.cu)
+TFGPU_LIB_PATH="$OUT/libtfhost_asan.so" LD_PRELOAD="$(gcc -print-file-name=libasan.so) $(gcc -print-file-name=libubsan.so)" \
+    ASAN_OPTIONS=detect_leaks=0:halt_on_error=1 UBSAN_OPTIONS=print_stacktrace=1:halt_on_error=1 \
+    python -m pytest tests/test_deflate.py -q -m "not gpu" -p no:cacheprovider -k "stream_helper"
 # the queue serializer batchers (host_plan.cu)
 TFGPU_LIB_PATH="$OUT/libtfhost_asan.so" LD_PRELOAD="$(gcc -print-file-name=libasan.so) $(gcc -print-file-name=libubsan.so)" \
     ASAN_OPTIONS=detect_leaks=0:halt_on_error=1 UBSAN_OPTIONS=print_stacktrace=1:halt_on_error=1 \

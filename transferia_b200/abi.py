@@ -95,6 +95,8 @@ def make_row_meta(id=None, lsn=None, commit_time=None, txid_offsets=None, txid_h
 
 TF_COL_LENS8, TF_COL_LENS16 = 1, 2
 TF_WIRE_SER_JSON, TF_WIRE_SER_CSV = 4, 5
+TF_WIRE_F_CLOSING_NEWLINE, TF_WIRE_F_ANY_AS_STRING = 0x100, 0x200
+TF_WIRE_F_GZIP, TF_WIRE_F_ZLIB = 0x400, 0x800     # the row text as one gzip member / zlib stream (include/tfgpu.h)
 TF_WIRE_DEBEZIUM = 6
 TF_ROWERR_DBZ_EMIT_HOST = 53
 TF_ROWERR_SINK_KIND_HOST = 54

@@ -11,6 +11,7 @@
 #include "kernels_n2f.cuh"
 #include "kernels_dbz.cuh"
 #include "kernels_json_out.cuh"
+#include "kernels_deflate.cuh"
 namespace tfk {
 void launch_k_strictify(dim3 grid, dim3 block, size_t smem, cudaStream_t s, StrictArgs a);
 void launch_k_filter(dim3 grid, dim3 block, size_t smem, cudaStream_t s, FilterArgs a);
@@ -52,5 +53,8 @@ void launch_k_dbz_pass2(dim3 grid, dim3 block, size_t smem, cudaStream_t s, DbzW
 void launch_k_json_sizes(dim3 grid, dim3 block, size_t smem, cudaStream_t s, JsonArgs a);
 void launch_k_json_write(dim3 grid, dim3 block, size_t smem, cudaStream_t s, JsonArgs a);
 cudaError_t dbz_kernels_init();   // dynamic shared memory limit of k_dbz_pass1
+void launch_k_deflate_chunks(dim3 grid, dim3 block, size_t smem, cudaStream_t s, DeflateArgs a);
+void launch_k_deflate_finish(dim3 grid, dim3 block, size_t smem, cudaStream_t s, DeflateArgs a);
+cudaError_t deflate_kernels_init();   // dynamic shared memory limit of k_deflate_chunks
 cudaError_t lz4_kernels_init();   // dynamic shared memory limits of k_lz4_frames / k_frame_seal
 }  // namespace tfk

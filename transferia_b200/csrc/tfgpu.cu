@@ -100,6 +100,7 @@ struct tfgpu_engine {
     DevBuf sel_stage; uint8_t* sel_host = nullptr; size_t sel_host_cap = 0; tfgpu_columnar* gather_pool = nullptr;
     uint64_t h2d_bytes = 0;                            // bytes stage_input has copied to the device since creation
     DevBuf json_sizes, dbz_keysz, dbz_meta, dbz_old, dbz_msgsz, old_arena, part_ids;
+    DevBuf defl_meta;                                  // deflate wire formats: look-back cells, chunk checksums, work counter
     DbzEmitArgs dbz{};                                 // set by tfgpu_emit_debezium for the TF_WIRE_DEBEZIUM branch of run_chain
     unsigned long long* lz_phases = nullptr;      // debug: per-phase cycle counters of k_lz4_frames
     void* work_json_sizes(uint64_t n) { json_sizes.ensure(n * 4 + 256); return json_sizes.p; }
@@ -354,6 +355,26 @@ uint32_t grid_cap(const tfgpu_engine* e, uint32_t tiles_upper, uint32_t nslots, 
     return std::max(1u, std::min(tiles_upper, std::max(want, 8u)));
 }
 
+// DEFLATE of `total` bytes of row text into e->wire as one gzip member / zlib stream (kernels_deflate.cuh); DState.wire_total
+// receives its length. The total is the one the host already read to size the text, so this adds no host sync.
+void run_deflate(tfgpu_engine* e, const uint8_t* text, uint64_t total, bool zlib) {
+    cudaStream_t s = e->stream;
+    const uint64_t nch = (total + DF_CHUNK - 1) / DF_CHUNK;
+    if (nch >= (1ull << 32)) throw tfplan::FatalError(TF_E_FATAL_ARG, "row text too large to compress in one call");
+    e->wire.ensure(total + nch * DF_CHUNK_OVERHEAD + 64);        // every chunk at most stored + marker, plus header, final block, trailer
+    Layout L;
+    const size_t o_pfx = L.take(nch * 8), o_sums = L.take(nch * 8), o_ticket = L.take(4);
+    e->defl_meta.ensure(L.total());
+    uint8_t* M = e->defl_meta.p;
+    CK(cudaMemsetAsync(M + o_pfx, 0, nch * 8, s)); CK(cudaMemsetAsync(M + o_ticket, 0, 4, s));
+    DeflateArgs da{text, total, e->wire.p, (unsigned long long*)(M + o_pfx), (uint32_t*)(M + o_sums), (uint32_t*)(M + o_ticket), (uint32_t)nch, zlib ? 1 : 0, e->d_state};
+    if (nch) {
+        const uint32_t grid = (uint32_t)std::min<uint64_t>(nch, (uint64_t)e->sm_count * 2);     // two CTAs of ~105 KiB per SM
+        e->prof_begin("k_deflate_chunks", s); launch_k_deflate_chunks(grid, DF_THREADS, df_smem().total, s, da); e->prof_end(s);
+    }
+    e->prof_begin("k_deflate_finish", s); launch_k_deflate_finish(1, 1024, 0, s, da); e->prof_end(s);
+}
+
 void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* dev_cols, const uint8_t* dev_kinds, int wire_fmt, const uint8_t* pre_err = nullptr) {
     const bool columnar = wire_fmt == TF_WIRE_COLUMNAR_INTERNAL;
     const tfplan::Plan& pl = pd.plan;
@@ -485,11 +506,13 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
         LayoutArgs lj{e->d_cols, 0, pd.d_out_cols, pd.d_str_slots, 1, e->tile_sum, e->tile_base, sz.ntiles_cap, pd.d_col_headers, pd.d_col_header_off,
                       e->raw.p, e->d_state, n, 1, e->frame_bytes, e->col_bytes};
         e->prof_begin("k_layout_scan", s); launch_k_layout_scan(1, 1024, 0, s, lj); e->prof_end(s);
+        uint64_t json_total = 0;
         {   // row text has no useful upper bound ('f' floats reach 300+ characters): size the output from the measured total
-            uint64_t total = 0; CK(cudaMemcpyAsync(&total, e->col_bytes, 8, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
-            e->raw.ensure(total + 256); ja.raw = e->raw.p;
+            CK(cudaMemcpyAsync(&json_total, e->col_bytes, 8, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
+            e->raw.ensure(json_total + 256); ja.raw = e->raw.p;
         }
         e->prof_begin("k_json_write", s); launch_k_json_write(jt ? jt : 1, TF_JSON_TILE, 0, s, ja); e->prof_end(s);
+        if (ser && (wire_fmt & (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB))) run_deflate(e, e->raw.p, n ? json_total : 0, (wire_fmt & TF_WIRE_F_ZLIB) != 0);
         CK(cudaGetLastError());
         return;
     }
@@ -575,7 +598,11 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
 
 
 // wire format ids accepted by the encode entry points; serializer formats need no sink in the plan
-static bool wire_is_ser(int wire_fmt) { const int b = wire_fmt & 0xff; return (b == TF_WIRE_SER_JSON || b == TF_WIRE_SER_CSV) && (wire_fmt & ~(0xff | TF_WIRE_F_CLOSING_NEWLINE | TF_WIRE_F_ANY_AS_STRING)) == 0; }
+static bool wire_is_ser(int wire_fmt) {
+    const int b = wire_fmt & 0xff;
+    return (b == TF_WIRE_SER_JSON || b == TF_WIRE_SER_CSV) && (wire_fmt & ~(0xff | TF_WIRE_F_CLOSING_NEWLINE | TF_WIRE_F_ANY_AS_STRING | TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB)) == 0 &&
+           (wire_fmt & (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB)) != (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB);
+}
 static bool wire_known(int wire_fmt) { return wire_fmt == TF_WIRE_CH_NATIVE || wire_fmt == TF_WIRE_CH_NATIVE_LZ4 || wire_fmt == TF_WIRE_CH_JSONEACHROW || wire_is_ser(wire_fmt); }
 
 extern "C" {
@@ -608,7 +635,7 @@ int tfgpu_engine_create(const char* cfg_json, const int* device_ids, int n_devic
         CK(cudaMalloc(&e->d_tail, 64)); CK(cudaMemset(e->d_tail, 0, 64));
         CK(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
         CK(cudaMalloc(&e->d_state, sizeof(DState)));
-        CK(lz4_kernels_init()); CK(dbz_kernels_init());
+        CK(lz4_kernels_init()); CK(dbz_kernels_init()); CK(deflate_kernels_init());
     } catch (const CudaError& c) { return c.e == cudaErrorMemoryAllocation ? TF_E_RETRY_OOM : TF_E_RETRY_LAUNCH; }
     catch (const std::exception&) { return TF_E_FATAL_CONFIG; }
     *out = e.release();
@@ -938,15 +965,16 @@ static void finish_wire(tfgpu_engine* e, uint64_t n, int wire_fmt, tfgpu_result*
     DState st; CK(cudaMemcpyAsync(&st, e->d_state, sizeof st, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
     r->rows_in = n; r->rows_out = st.n_kept; r->raw_len = st.raw_total;
     const bool lz = wire_fmt == TF_WIRE_CH_NATIVE_LZ4;
+    const bool wire = lz || (wire_fmt & (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB));      // compressed: the bytes are in e->wire
     r->n_frames = lz ? st.n_frames : 0;
-    r->bytes_len = lz ? st.wire_total : st.raw_total;
+    r->bytes_len = wire ? st.wire_total : st.raw_total;
     if (e->pinned_cap < r->bytes_len + 64) {   // grow-only pinned landing buffer, owned by the engine
         if (e->pinned) { CK(cudaFreeHost(e->pinned)); e->pinned = nullptr; e->pinned_cap = 0; }
         const size_t want = align_up(r->bytes_len + r->bytes_len / 4 + 4096, 1 << 20);
         CK(cudaMallocHost(&e->pinned, want)); e->pinned_cap = want;
     }
     r->bytes = e->pinned; r->bytes_pinned = false;
-    CK(cudaMemcpyAsync(r->bytes, lz ? e->wire.p : e->raw.p, r->bytes_len, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(r->bytes, wire ? e->wire.p : e->raw.p, r->bytes_len, cudaMemcpyDeviceToHost, s));
     { const int b = wire_fmt & 0xff;
       if ((b == TF_WIRE_SER_JSON || b == TF_WIRE_SER_CSV || b == TF_WIRE_CH_JSONEACHROW || b == TF_WIRE_DEBEZIUM) && st.n_kept) { r->row_sizes.resize(st.n_kept); CK(cudaMemcpyAsync(r->row_sizes.data(), e->json_sizes.p, st.n_kept * 4, cudaMemcpyDeviceToHost, s)); }
       if (b == TF_WIRE_DEBEZIUM && st.n_kept) { r->key_sizes.resize(st.n_kept); CK(cudaMemcpyAsync(r->key_sizes.data(), e->dbz_keysz.p, st.n_kept * 4, cudaMemcpyDeviceToHost, s));

@@ -84,6 +84,10 @@ def load_library():
     L.tfgpu_engine_launch_count.argtypes = [vp]; L.tfgpu_engine_launch_count.restype = u64
     L.tfgpu_profile_enable.argtypes = [vp, i]
     L.tfgpu_profile_read.argtypes = [vp]; L.tfgpu_profile_read.restype = cp
+    L.tfgpu_deflate_stream_open.argtypes = [i, C.POINTER(vp)]
+    L.tfgpu_deflate_stream_append.argtypes = [vp, vp, u64, u64, vp, u64, C.POINTER(u64)]
+    L.tfgpu_deflate_stream_close.argtypes = [vp, vp, u64, C.POINTER(u64)]
+    L.tfgpu_deflate_stream_free.argtypes = [vp]; L.tfgpu_deflate_stream_free.restype = None
     _lib = L
     return L
 
@@ -95,7 +99,39 @@ EXPORTED_SYMBOLS = [
     "tfgpu_result_n_errors", "tfgpu_result_errors", "tfgpu_result_batch", "tfgpu_result_bytes",
     "tfgpu_result_bytes_len", "tfgpu_result_raw_len", "tfgpu_result_n_frames", "tfgpu_result_release",
     "tfgpu_engine_launch_count", "tfgpu_profile_enable", "tfgpu_profile_read",
+    "tfgpu_deflate_stream_open", "tfgpu_deflate_stream_append", "tfgpu_deflate_stream_close", "tfgpu_deflate_stream_free",
 ]
+
+
+class DeflateStream:
+    """One gzip member / zlib stream out of the results of several TF_WIRE_F_GZIP / TF_WIRE_F_ZLIB pushes (host only):
+    append(result bytes, raw_len) returns the bytes to write next, close() the final block and trailer."""
+
+    def __init__(self, container: int):
+        self._L = load_library()
+        self._h = C.c_void_p()
+        rc = self._L.tfgpu_deflate_stream_open(container, C.byref(self._h))
+        if rc != 0:
+            raise EngineError(rc, "tfgpu_deflate_stream_open: container must be TF_WIRE_F_GZIP or TF_WIRE_F_ZLIB")
+
+    def append(self, data: bytes, raw_len: int) -> bytes:
+        out = C.create_string_buffer(len(data) + 16); n = C.c_uint64()
+        rc = self._L.tfgpu_deflate_stream_append(self._h, data, len(data), raw_len, out, len(out), C.byref(n))
+        if rc != 0:
+            raise EngineError(rc, "tfgpu_deflate_stream_append: the result's framing does not match the stream's container")
+        return out.raw[:n.value]
+
+    def close(self) -> bytes:
+        out = C.create_string_buffer(32); n = C.c_uint64()
+        rc = self._L.tfgpu_deflate_stream_close(self._h, out, len(out), C.byref(n))
+        if rc != 0:
+            raise EngineError(rc, "tfgpu_deflate_stream_close")
+        return out.raw[:n.value]
+
+    def __del__(self):
+        if getattr(self, "_h", None):
+            self._L.tfgpu_deflate_stream_free(self._h)
+            self._h = None
 
 
 def debezium_table_schema(schema_text: str):
