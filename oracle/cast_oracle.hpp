@@ -189,6 +189,13 @@ inline int strictify_value(const GoVal& v, int tf, GoVal& out) {
     case TF_FLOAT: {                                                              // cast.ToFloat32E: strings through ParseFloat(s, 32)
         if (v.k == INT) { out.k = F32; out.f = (double)(float)v.i; return OK; }      // float32(s): one conversion, not two
         if (v.k == UINT) { out.k = F32; out.f = (double)(float)v.u; return OK; }
+        if (v.k == STRING) {                                                      // ParseFloat(s, 32): one rounding; a range error is cast's error
+            double f; const int rc = jsn::go_parse_float(v.s, f); if (rc) return CAST_ERR;      // syntax, and overflow of float64 itself
+            if (!std::isfinite(f)) { out.k = F32; out.f = f; return OK; }                       // inf / infinity / nan spellings
+            std::string t = v.s; t.erase(std::remove(t.begin(), t.end(), '_'), t.end());
+            const float g = std::strtof(t.c_str(), nullptr); if (std::isinf(g)) return CAST_ERR;
+            out.k = F32; out.f = g; return OK;
+        }
         double f; const int rc = cast_to_f64(v, f); if (rc) return rc;
         out.k = F32; out.f = (double)(float)f; return OK;
     }

@@ -202,7 +202,8 @@ inline int csv_convert(const CsvOpts& o, int tf, const std::string& cell, uint8_
     }
     case TF_FLOAT: case TF_DOUBLE: {    // parseFloatValue (DecimalPoint unset) -> cast.ToFloat32E / castx.ToJSONNumberE -> Float64()
         double d; int rc = parse_float_fast(p, n, d); if (rc) return rc == 2 ? CSV_UNSUPPORTED : CSV_BAD_FLOAT;
-        if (tf == TF_FLOAT) { float f = (float)d; std::memcpy(val, &f, 4); } else std::memcpy(val, &d, 8);
+        // cast.ToFloat32E(string) is strconv.ParseFloat(s, 32): one rounding to binary32 (glibc strtof), not float32(float64)
+        if (tf == TF_FLOAT) { float f = std::strtof(cell.c_str(), nullptr); std::memcpy(val, &f, 4); } else std::memcpy(val, &d, 8);
         return 0;
     }
     default: break;

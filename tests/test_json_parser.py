@@ -83,7 +83,7 @@ ALL_FIELDS = [{"name": "i8", "type": "int8"}, {"name": "i64", "type": "int64"}, 
 QUIRK_VALUES = [
     b"null", b"0", b"-1", b"127", b"128", b"-129", b"300", b"1.5", b"1e3", b"1E+2", b"-0", b"0.1", b"123456789012345678", b"1234567890123456789", b"9223372036854775807",
     b"9223372036854775808", b"18446744073709551615", b"18446744073709551616", b"-9223372036854775808", b"12345678765432.23456765432", b"0.8444218515250481",
-    b"2.2250738585072014e-308", b"1.7976931348623157e308", b"1e400", b"1e-400", b"4.9e-324", b"1.", b".5", b"-.5", b"-", b"+1", b"1.2.3", b"e", b"1e", b"--1", b"inf", b"-inf", b"nan", b"NaN", b"+Inf",
+    b"2.2250738585072014e-308", b"1.7976931348623157e308", b"1e400", b"1e-400", b"4.9e-324", b"1.", b"-1.", b".5", b"-.5", b"-", b"+1", b"1.2.3", b"e", b"1e", b"--1", b"inf", b"-inf", b"nan", b"NaN", b"+Inf",
     b"true", b"false", b'"abc"', b'""', b'"12"', b'"0x1f"', b'"017"', b'"1_000"', b'"-5"', b'"1e2"', b'"1.25"', b'"true"', b'"T"', b'"maybe"', b'"inf"', b'"nan"', b'"+nan"', b'"0x1p-2"',
     b'"a\\nb\\t\\"q\\" \\\\ \\/ \\u0041\\u00e9\\u20ac\\ud83d\\ude00 \\ud83d x \\udc00 \\uZZZZ \\u12"', b'"\\x \\a"', b'"<tag> & \\u2028 \\u0000"', b'"\xd0\xbf\xd1\x80\xd0\xb8\xd0\xb2\xd0\xb5\xd1\x82 \xff\xfe"',
     b'"dGVzdA=="', b'"dGVzdDI="', b'"dGVz\\ndA=="', b'"dGVzdA="', b'"dGVzdA==="', b'"d"', b'"dG"', b'"dG=="', b'"dGV="', b'"dGVzd A=="', b'"4pyTIMOgIGxhIG1vZGU="',

@@ -156,8 +156,9 @@ static __device__ int d_parse_bool(const uint8_t* s, uint32_t n, bool& out) {   
     return 1;
 }
 __constant__ double d_p10[23] = {1e0, 1e1, 1e2, 1e3, 1e4, 1e5, 1e6, 1e7, 1e8, 1e9, 1e10, 1e11, 1e12, 1e13, 1e14, 1e15, 1e16, 1e17, 1e18, 1e19, 1e20, 1e21, 1e22};
-// decimal text -> double, exact when <= 15 significant digits and |exp10| <= 22 (one correctly rounded IEEE op); rc 2 otherwise
-static __device__ int d_parse_float(const uint8_t* s, uint32_t n, double& out) {
+// decimal text -> double, exact when <= 15 significant digits and |exp10| <= 22 (one correctly rounded IEEE op); rc 2 otherwise.
+// f32 (optional): the same text rounded once to binary32, as strconv.ParseFloat(s, 32) does, not through the double
+static __device__ int d_parse_float(const uint8_t* s, uint32_t n, double& out, float* f32 = nullptr) {
     uint32_t i = 0; bool neg = false;
     if (!n) return 1;
     if (s[0] == '+' || s[0] == '-') { neg = s[0] == '-'; i = 1; }
@@ -178,10 +179,23 @@ static __device__ int d_parse_float(const uint8_t* s, uint32_t n, double& out) {
     }
     if (i != n) return (s[i] == '_' || (s[i] | 0x20) == 'x' || (s[i] | 0x20) == 'p') ? 2 : 1;
     e += dp;
-    if (m == 0) { out = neg ? -0.0 : 0.0; return 0; }
+    if (m == 0) { out = neg ? -0.0 : 0.0; if (f32) *f32 = neg ? -0.0f : 0.0f; return 0; }
     if (nd > 15 || e < -22 || e > 22) return 2;
-    double d = (double)m; d = e < 0 ? __ddiv_rn(d, d_p10[-e]) : __dmul_rn(d, d_p10[e]);
-    out = neg ? -d : d; return 0;
+    const double md = (double)m, p = d_p10[e < 0 ? -e : e];
+    const double d = e < 0 ? __ddiv_rn(md, p) : __dmul_rn(md, p);
+    out = neg ? -d : d;
+    if (f32) {
+        // Rounding d again to binary32 errs only when d sits exactly on a binary32 midpoint (low 29 mantissa bits 1 << 28)
+        // while m * 10^e does not. m < 2^50 and 10^|e| are exact, so one fma gives the exact residual, whose sign picks the
+        // side; a zero residual is a true midpoint and ties to even. Values here lie in [1e-22, 1e37]: binary32 normals.
+        float f = __double2float_rn(d);
+        if ((__double_as_longlong(d) & 0x1FFFFFFFll) == (1ll << 28)) {
+            const double r = e < 0 ? __fma_rn(-d, p, md) : __fma_rn(md, p, -d);       // sign of m * 10^e - d
+            if (r > 0) f = __double2float_ru(d); else if (r < 0) f = __double2float_rd(d);
+        }
+        *f32 = neg ? -f : f;
+    }
+    return 0;
 }
 __device__ __forceinline__ int64_t d_days_from_civil(int64_t y, unsigned m, unsigned d) {
     y -= m <= 2;
@@ -261,8 +275,8 @@ static __device__ int csv_cell(const CsvArgs& a, const CsvColDev& c, uint64_t ro
         csv_store_fixed(c, row, (uint64_t)sec, nsec); return 0;
     }
     case TF_FLOAT: case TF_DOUBLE: {
-        double d; const int rc = d_parse_float(p, n, d); if (rc) return rc == 2 ? CSV_UNSUPPORTED : CSV_BAD_FLOAT;
-        if (c.tf == TF_FLOAT) { const float f = (float)d; csv_store_fixed(c, row, __float_as_uint(f), 0); } else csv_store_fixed(c, row, (uint64_t)__double_as_longlong(d), 0);
+        double d; float f; const int rc = d_parse_float(p, n, d, c.tf == TF_FLOAT ? &f : nullptr); if (rc) return rc == 2 ? CSV_UNSUPPORTED : CSV_BAD_FLOAT;
+        if (c.tf == TF_FLOAT) csv_store_fixed(c, row, __float_as_uint(f), 0); else csv_store_fixed(c, row, (uint64_t)__double_as_longlong(d), 0);
         return 0;
     }
     }
