@@ -16,6 +16,8 @@ from transferia_b200 import abi, dispatch, engine, workload
 
 
 def test_library_exports_every_declared_symbol():
+    """Every function the headers declare has one prototype in the binding's table of its header, with the header's parameter count, and
+    the library exports it with that prototype applied."""
     from transferia_b200 import sink
     hdr = "".join(open(os.path.join(ROOT, "include", h)).read() for h in sorted(os.listdir(os.path.join(ROOT, "include"))) if h.endswith(".h"))
     hdr = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
@@ -26,6 +28,18 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(L, name), name
     assert L.tfgpu_version().decode().startswith("tfgpu ") and b"sm_90a" in L.tfgpu_version()
+    proto = r"^\s*(?:const\s+)?\w+(?:\s*\*)?\s+(tfgpu_\w+)\s*\(([^;{]*?)\)\s*;"
+    for h, table in (("tfgpu.h", abi.TFGPU_H_PROTOTYPES), ("tfgpu_sink.h", abi.TFGPU_SINK_H_PROTOTYPES)):
+        text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", h)).read(), flags=re.S)
+        params = dict(re.findall(proto, text, flags=re.M | re.S))
+        assert set(params) == set(re.findall(r"\b(tfgpu_\w+)\s*\(", text)) == set(table), (h, set(params) ^ set(table))
+        for name, args in params.items():
+            n = 0 if args.strip() in ("", "void") else args.count(",") + 1
+            assert len(table[name][1]) == n, (name, table[name][1], args)
+    assert abi.PROTOTYPES == {**abi.TFGPU_H_PROTOTYPES, **abi.TFGPU_SINK_H_PROTOTYPES}
+    for name, (restype, argtypes) in abi.PROTOTYPES.items():
+        f = getattr(L, name)
+        assert f.restype is restype and list(f.argtypes) == argtypes, name
 
 
 def test_library_is_sm90a_native():
@@ -451,7 +465,6 @@ def test_transformation_test_multiple_transformers(po):
 def test_headers_are_plain_c(tmp_path):
     """The boundary is a C ABI: both headers compile as C99 (`gcc -std=c99 -pedantic`), and the struct sizes the Python binding assumes are the
     ones the C compiler lays out."""
-    from transferia_b200 import rows, sink
     src = tmp_path / "hdr.c"
     src.write_text('#include <stdio.h>\n#include "tfgpu.h"\n#include "tfgpu_sink.h"\n'
                    'int main(void) { printf("%zu %zu %zu %zu %zu %zu %zu\\n", sizeof(tf_col), sizeof(tf_batch), sizeof(tf_item), sizeof(tf_rows), sizeof(tf_table),'
@@ -459,7 +472,7 @@ def test_headers_are_plain_c(tmp_path):
     exe = tmp_path / "hdr"
     subprocess.run(["gcc", "-std=c99", "-Wall", "-Wextra", "-pedantic", "-Werror", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
     got = [int(x) for x in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
-    want = [C.sizeof(abi.TfCol), C.sizeof(abi.TfBatch), C.sizeof(rows.TfItem), C.sizeof(rows.TfRows), C.sizeof(rows.TfTable), C.sizeof(sink.TfSinkEvent), C.sizeof(sink.TfSinkStats)]
+    want = [C.sizeof(abi.TfCol), C.sizeof(abi.TfBatch), C.sizeof(abi.TfItem), C.sizeof(abi.TfRows), C.sizeof(abi.TfTable), C.sizeof(abi.TfSinkEvent), C.sizeof(abi.TfSinkStats)]
     assert got == want, (got, want)
 
 

@@ -1,4 +1,4 @@
-"""ctypes view of include/tfgpu.h: the columnar batch that crosses the C-ABI.
+"""ctypes view of include/tfgpu.h and include/tfgpu_sink.h: the structs that cross the C-ABI and the prototype of every function.
 
 This module only describes memory; it computes nothing.  The engine binding
 (transferia_b200.engine) uses it, and so do the tests' CPU checker and the workload generator,
@@ -7,6 +7,7 @@ because they all speak the same `tf_batch` struct.
 from __future__ import annotations
 
 import ctypes as C
+import json
 from dataclasses import dataclass, field
 from typing import Any, List, Optional, Sequence
 
@@ -77,6 +78,11 @@ class TfRowMeta(C.Structure):
 class TfOldKeys(C.Structure):
     """tf_old_keys: ChangeItem.OldKeys of a batch as a second set of typed columns (old_keys.go:3-7)."""
     _fields_ = [("values", C.c_void_p), ("present_cols", C.c_void_p), ("row_has", C.c_void_p)]
+
+
+def schema_json(schema) -> str:
+    """A table schema as the ColSchema JSON array the calls take: JSON text as it is, or ColSchema dicts without their "_" keys."""
+    return schema if isinstance(schema, str) else json.dumps([{k: v for k, v in c.items() if not k.startswith("_")} for c in schema])
 
 
 def make_old_keys(old_batch, present_cols, row_has=None):
@@ -295,3 +301,131 @@ def fixed_to_column(tf_type: int, values: Sequence, nulls: Optional[Sequence[boo
         validity = pack_validity(~np.asarray(nulls, dtype=bool))
     aux = None if nanos is None else np.asarray(nanos, dtype=np.uint32)
     return Column(tf_type, values=arr, validity=validity, aux=aux)
+
+
+# ------------------------------------------------------------------ include/tfgpu_sink.h
+class TfTable(C.Structure):
+    _fields_ = [("schema", C.c_char_p), ("table", C.c_char_p), ("schema_json", C.c_char_p)]
+
+
+class TfItem(C.Structure):
+    _fields_ = [("lsn", C.c_uint64), ("commit_time", C.c_uint64), ("size_read", C.c_uint64), ("size_values", C.c_uint64), ("values_off", C.c_uint64), ("old_keys_off", C.c_uint64),
+                ("id", C.c_uint32), ("table", C.c_uint32), ("n_values", C.c_uint32), ("txid_off", C.c_uint32), ("txid_len", C.c_uint32),
+                ("part_off", C.c_uint32), ("part_len", C.c_uint32), ("counter", C.c_int32), ("kind", C.c_uint8), ("flags", C.c_uint8), ("pad", C.c_uint8 * 2)]
+
+
+class TfRows(C.Structure):
+    _fields_ = [("n_items", C.c_uint64), ("items", C.POINTER(TfItem)), ("n_tables", C.c_uint32), ("pad", C.c_uint32), ("tables", C.POINTER(TfTable)),
+                ("values", C.c_void_p), ("values_len", C.c_uint64), ("strings", C.c_void_p), ("strings_len", C.c_uint64)]
+
+
+class TfSinkEvent(C.Structure):
+    _fields_ = [("type", C.c_int32), ("table", C.c_uint32), ("out_schema", C.c_char_p), ("out_table", C.c_char_p), ("n_items", C.c_uint64),
+                ("item_idx", C.POINTER(C.c_uint64)), ("errors", C.c_void_p), ("batch", C.c_void_p), ("wire", C.c_void_p),
+                ("wire_len", C.c_uint64), ("raw_len", C.c_uint64), ("n_frames", C.c_uint64), ("msg_sizes", C.POINTER(C.c_uint32)), ("plan_id", C.c_int32), ("pad", C.c_int32)]
+
+
+class TfSinkStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("pushes", "downstream_pushes", "change_items_pushed", "row_events_pushed", "inflight_bytes", "filter_dropped",
+                                          "transform_dropped", "transform_errors", "max_commit_time", "min_commit_time", "without_commit_time", "wire_bytes",
+                                          "metering_input_rows", "metering_output_rows")]
+
+
+TF_SINK_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(TfSinkEvent))      # tf_sink_fn
+
+
+# ------------------------------------------------------------------ every function of both headers
+# name -> (restype, argtypes), one table per header; engine.load_library() applies PROTOTYPES (both) once. Handles are void*, char buffers char*, byte and integer arrays
+# void* (numpy addresses, bytes and string buffers pass as they are); structs go by their class, and scalars, scalar out-parameters and
+# returned arrays at the header's width.
+_v, _s, _i, _u32, _u64, _P = C.c_void_p, C.c_char_p, C.c_int, C.c_uint32, C.c_uint64, C.POINTER
+TFGPU_H_PROTOTYPES = {
+    "tfgpu_engine_create": (_i, [_s, _P(_i), _i, _P(_v)]),
+    "tfgpu_engine_destroy": (_i, [_v]),
+    "tfgpu_last_error": (_s, [_v]),
+    "tfgpu_engine_set_stream": (_i, [_v, _v]),
+    "tfgpu_plan": (_i, [_v, _s, _s, _s, _s, _s, _P(_i)]),
+    "tfgpu_plan_validate": (_i, [_s, _s, _s, _s, _s, _s, _u64, _s, _u64]),
+    "tfgpu_plan_describe": (_s, [_v, _i]),
+    "tfgpu_push_columns": (_i, [_v, _i, _P(TfBatch), _P(_v)]),
+    "tfgpu_push_encode": (_i, [_v, _i, _i, _P(TfBatch), _P(_v)]),
+    "tfgpu_push_encode_selective": (_i, [_v, _i, _i, _P(TfBatch), _i, _P(_v)]),
+    "tfgpu_engine_h2d_bytes": (_u64, [_v]),
+    "tfgpu_emit_debezium": (_i, [_v, _i, _s, _P(TfBatch), _P(TfRowMeta), _P(_v)]),
+    "tfgpu_emit_debezium_crud": (_i, [_v, _i, _s, _P(TfBatch), _P(TfOldKeys), _P(TfRowMeta), _P(_v)]),
+    "tfgpu_result_dbz_msg_sizes": (_P(_u32), [_v]),
+    "tfgpu_emit_debezium_validate": (_i, [_s, _s, _s, _s, _s, _s, _u64, _s, _u64]),
+    "tfgpu_measure": (_i, [_v, _P(TfBatch), _v, _P(_u64)]),
+    "tfgpu_parse_csv": (_i, [_v, _i, _s, _v, _u64, _i, _i, _P(_v)]),
+    "tfgpu_result_consumed": (_u64, [_v]),
+    "tfgpu_push_encode_resident": (_i, [_v, _i, _i, _P(TfBatch)]),
+    "tfgpu_resident_stats": (_i, [_v, _P(_u64), _P(_u64), _P(_u64), _P(_u64)]),
+    "tfgpu_resident_fetch": (_i, [_v, _i, _v, _u64]),
+    "tfgpu_result_rows_in": (_u64, [_v]),
+    "tfgpu_parse_json": (_i, [_v, _i, _s, _v, _u64, _i, _P(TfMsg), _u32, _i, _P(_v)]),
+    "tfgpu_parse_debezium": (_i, [_v, _i, _s, _v, _u64, _i, _v, _u32, _i, _P(_v)]),
+    "tfgpu_debezium_schema_validate": (_i, [_s, _s, _u64, _s, _u64]),
+    "tfgpu_debug_lz4_phases": (_i, [_v, _i, _P(_u64)]),
+    "tfgpu_result_selection": (_P(_u32), [_v]),
+    "tfgpu_result_meta_kinds": (_P(C.c_uint8), [_v]),
+    "tfgpu_result_meta_tx_id": (_P(_u32), [_v]),
+    "tfgpu_result_meta_lsn": (_P(_u64), [_v]),
+    "tfgpu_result_meta_commit_time": (_P(_u64), [_v]),
+    "tfgpu_result_rows_out": (_u64, [_v]),
+    "tfgpu_result_n_errors": (_u64, [_v]),
+    "tfgpu_result_errors": (_P(TfRowErr), [_v]),
+    "tfgpu_result_batch": (_P(TfBatch), [_v]),
+    "tfgpu_result_bytes": (_v, [_v]),
+    "tfgpu_result_bytes_len": (_u64, [_v]),
+    "tfgpu_result_raw_len": (_u64, [_v]),
+    "tfgpu_result_n_frames": (_u64, [_v]),
+    "tfgpu_result_row_sizes": (_P(_u32), [_v]),
+    "tfgpu_result_part_ids": (_P(_u32), [_v]),
+    "tfgpu_result_key_sizes": (_P(_u32), [_v]),
+    "tfgpu_queue_json_batches": (_i, [_v, _u64, _u64, _u64, _v, _u64, _P(_u64)]),
+    "tfgpu_queue_debezium_batches": (_i, [_v, _u64, _u64, _v, _u64, _P(_u64)]),
+    "tfgpu_result_release": (None, [_v]),
+    "tfgpu_deflate_stream_open": (_i, [_i, _P(_v)]),
+    "tfgpu_deflate_stream_append": (_i, [_v, _v, _u64, _u64, _v, _u64, _P(_u64)]),
+    "tfgpu_deflate_stream_close": (_i, [_v, _v, _u64, _P(_u64)]),
+    "tfgpu_deflate_stream_free": (None, [_v]),
+    "tfgpu_engine_launch_count": (_u64, [_v]),
+    "tfgpu_profile_enable": (_i, [_v, _i]),
+    "tfgpu_profile_read": (_s, [_v]),
+    "tfgpu_version": (_s, []),
+}
+TFGPU_SINK_H_PROTOTYPES = {
+    "tfgpu_ch_open": (_i, [_i, _s, _P(_v)]),
+    "tfgpu_ch_close": (_i, [_v]),
+    "tfgpu_ch_last_error": (_s, [_v]),
+    "tfgpu_ch_server_info": (_s, [_v]),
+    "tfgpu_ch_exception_code": (_i, [_v]),
+    "tfgpu_ch_insert_begin": (_i, [_v, _s, _s, _s]),
+    "tfgpu_ch_insert_columns": (_s, [_v]),
+    "tfgpu_ch_insert_data": (_i, [_v, _v, _u64]),
+    "tfgpu_ch_insert_end": (_i, [_v, _P(_u64), _P(_u64)]),
+    "tfgpu_ch_stats": (_i, [_v, _P(_u64), _P(_u64), _P(_u64)]),
+    "tfgpu_ch_insert_query": (C.c_int64, [_s, _s, _s, _i, _s, _u64]),
+    "tfgpu_columnar_create": (_i, [_P(_v)]),
+    "tfgpu_columnar_destroy": (_i, [_v]),
+    "tfgpu_columnar_last_error": (_s, [_v]),
+    "tfgpu_rows_to_batch": (_i, [_v, _P(TfRows), _u32, _v, _u64, _i, _P(_P(TfBatch)), _P(_P(TfRowMeta)), _P(_P(TfOldKeys))]),
+    "tfgpu_batch_to_rows": (_i, [_P(TfBatch), _v, _u64, _v, _P(_u64)]),
+    "tfgpu_batch_gather": (_i, [_v, _P(TfBatch), _v, _i, _P(_P(TfBatch)), _P(_P(_u32))]),
+    "tfgpu_batch_gather_sel": (_i, [_v, _P(TfBatch), _v, _u64, _i, _P(_P(TfBatch))]),
+    "tfgpu_sink_create": (_i, [_v, _s, _P(_v)]),
+    "tfgpu_sink_destroy": (_i, [_v]),
+    "tfgpu_sink_last_error": (_s, [_v]),
+    "tfgpu_sink_set_callback": (_i, [_v, TF_SINK_FN, _v]),
+    "tfgpu_sink_set_clickhouse": (_i, [_v, _v]),
+    "tfgpu_sink_push": (_i, [_v, _P(TfRows)]),
+    "tfgpu_sink_stats": (_i, [_v, _P(TfSinkStats)]),
+    "tfgpu_dispatcher_create": (_i, [_P(_v), _i, _P(_v)]),
+    "tfgpu_dispatcher_submit": (_i, [_v, _P(TfRows), _P(_u64)]),
+    "tfgpu_dispatcher_wait": (_i, [_v, _u64]),
+    "tfgpu_dispatcher_drain": (_i, [_v]),
+    "tfgpu_dispatcher_destroy": (_i, [_v]),
+    "tfgpu_host_cityhash128": (None, [_v, _u64, _P(_u64)]),
+    "tfgpu_regex_replace_all": (C.c_int64, [_s, _s, _v, _u64, _v, _u64]),
+}
+PROTOTYPES = {**TFGPU_H_PROTOTYPES, **TFGPU_SINK_H_PROTOTYPES}

@@ -15,7 +15,9 @@ import ctypes as C
 import json
 import os
 from dataclasses import dataclass
-from typing import List, Optional, Tuple
+from typing import Any, List, Optional, Tuple
+
+import numpy as np
 
 from . import abi
 
@@ -38,7 +40,7 @@ _lib = None
 
 
 def load_library():
-    """dlopen transferia_b200/libtfgpu.so and declare every symbol of include/tfgpu.h."""
+    """dlopen transferia_b200/libtfgpu.so and give every function of include/tfgpu.h and include/tfgpu_sink.h its prototype."""
     global _lib
     if _lib is not None:
         return _lib
@@ -46,61 +48,14 @@ def load_library():
         raise RuntimeError(f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` — "
                            "the engine has no CPU fallback")
     L = C.CDLL(LIB_PATH)
-    vp, cp, i, u64 = C.c_void_p, C.c_char_p, C.c_int, C.c_uint64
-    L.tfgpu_version.restype = cp
-    L.tfgpu_engine_create.argtypes = [cp, C.POINTER(C.c_int), i, C.POINTER(vp)]
-    L.tfgpu_engine_destroy.argtypes = [vp]
-    L.tfgpu_last_error.argtypes = [vp]; L.tfgpu_last_error.restype = cp
-    L.tfgpu_engine_set_stream.argtypes = [vp, vp]
-    L.tfgpu_plan.argtypes = [vp, cp, cp, cp, cp, cp, C.POINTER(C.c_int)]
-    L.tfgpu_plan_describe.argtypes = [vp, i]; L.tfgpu_plan_describe.restype = cp
-    L.tfgpu_plan_validate.argtypes = [cp, cp, cp, cp, cp, cp, u64, cp, u64]
-    L.tfgpu_push_columns.argtypes = [vp, i, C.POINTER(abi.TfBatch), C.POINTER(vp)]
-    L.tfgpu_push_encode.argtypes = [vp, i, i, C.POINTER(abi.TfBatch), C.POINTER(vp)]
-    L.tfgpu_push_encode_selective.argtypes = [vp, i, i, C.POINTER(abi.TfBatch), i, C.POINTER(vp)]
-    L.tfgpu_engine_h2d_bytes.argtypes = [vp]; L.tfgpu_engine_h2d_bytes.restype = u64
-    L.tfgpu_parse_csv.argtypes = [vp, i, cp, vp, u64, i, i, C.POINTER(vp)]
-    L.tfgpu_result_row_sizes.argtypes = [vp]; L.tfgpu_result_row_sizes.restype = C.POINTER(C.c_uint32)
-    L.tfgpu_result_key_sizes.argtypes = [vp]; L.tfgpu_result_key_sizes.restype = C.POINTER(C.c_uint32)
-    L.tfgpu_result_part_ids.argtypes = [vp]; L.tfgpu_result_part_ids.restype = C.POINTER(C.c_uint32)
-    L.tfgpu_emit_debezium.argtypes = [vp, i, cp, C.POINTER(abi.TfBatch), C.POINTER(abi.TfRowMeta), C.POINTER(vp)]
-    L.tfgpu_queue_json_batches.argtypes = [vp, u64, u64, u64, vp, u64, C.POINTER(u64)]
-    L.tfgpu_parse_debezium.argtypes = [vp, i, cp, vp, u64, i, vp, C.c_uint32, i, C.POINTER(vp)]
-    for fn, ty in (("tfgpu_result_selection", C.c_uint32), ("tfgpu_result_meta_kinds", C.c_uint8), ("tfgpu_result_meta_tx_id", C.c_uint32), ("tfgpu_result_meta_lsn", u64), ("tfgpu_result_meta_commit_time", u64)):
-        getattr(L, fn).argtypes = [vp]; getattr(L, fn).restype = C.POINTER(ty)
-    L.tfgpu_debug_lz4_phases.argtypes = [vp, i, C.POINTER(u64)]
-    L.tfgpu_measure.argtypes = [vp, C.POINTER(abi.TfBatch), vp, C.POINTER(u64)]
-    L.tfgpu_parse_json.argtypes = [vp, i, cp, vp, u64, i, C.POINTER(abi.TfMsg), C.c_uint32, i, C.POINTER(vp)]
-    L.tfgpu_result_consumed.argtypes = [vp]; L.tfgpu_result_consumed.restype = u64
-    L.tfgpu_push_encode_resident.argtypes = [vp, i, i, C.POINTER(abi.TfBatch)]
-    L.tfgpu_resident_stats.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
-    L.tfgpu_resident_fetch.argtypes = [vp, i, vp, u64]
-    for name in ("rows_in", "rows_out", "n_errors", "bytes_len", "raw_len", "n_frames"):
-        f = getattr(L, "tfgpu_result_" + name); f.argtypes = [vp]; f.restype = u64
-    L.tfgpu_result_errors.argtypes = [vp]; L.tfgpu_result_errors.restype = C.POINTER(abi.TfRowErr)
-    L.tfgpu_result_batch.argtypes = [vp]; L.tfgpu_result_batch.restype = C.POINTER(abi.TfBatch)
-    L.tfgpu_result_bytes.argtypes = [vp]; L.tfgpu_result_bytes.restype = vp
-    L.tfgpu_result_release.argtypes = [vp]; L.tfgpu_result_release.restype = None
-    L.tfgpu_engine_launch_count.argtypes = [vp]; L.tfgpu_engine_launch_count.restype = u64
-    L.tfgpu_profile_enable.argtypes = [vp, i]
-    L.tfgpu_profile_read.argtypes = [vp]; L.tfgpu_profile_read.restype = cp
-    L.tfgpu_deflate_stream_open.argtypes = [i, C.POINTER(vp)]
-    L.tfgpu_deflate_stream_append.argtypes = [vp, vp, u64, u64, vp, u64, C.POINTER(u64)]
-    L.tfgpu_deflate_stream_close.argtypes = [vp, vp, u64, C.POINTER(u64)]
-    L.tfgpu_deflate_stream_free.argtypes = [vp]; L.tfgpu_deflate_stream_free.restype = None
+    for name, (restype, argtypes) in abi.PROTOTYPES.items():
+        f = getattr(L, name)
+        f.restype, f.argtypes = restype, argtypes
     _lib = L
     return L
 
 
-EXPORTED_SYMBOLS = [
-    "tfgpu_version", "tfgpu_engine_create", "tfgpu_engine_destroy", "tfgpu_last_error", "tfgpu_engine_set_stream",
-    "tfgpu_push_encode_selective", "tfgpu_engine_h2d_bytes", "tfgpu_plan", "tfgpu_plan_validate", "tfgpu_plan_describe", "tfgpu_push_columns", "tfgpu_push_encode", "tfgpu_parse_csv", "tfgpu_parse_json", "tfgpu_measure", "tfgpu_emit_debezium", "tfgpu_emit_debezium_crud", "tfgpu_result_dbz_msg_sizes", "tfgpu_emit_debezium_validate", "tfgpu_result_key_sizes", "tfgpu_result_part_ids", "tfgpu_result_row_sizes", "tfgpu_queue_json_batches", "tfgpu_queue_debezium_batches", "tfgpu_parse_debezium", "tfgpu_debezium_schema_validate", "tfgpu_debug_lz4_phases", "tfgpu_result_selection", "tfgpu_result_meta_kinds", "tfgpu_result_meta_tx_id", "tfgpu_result_meta_lsn", "tfgpu_result_meta_commit_time", "tfgpu_result_consumed", "tfgpu_push_encode_resident",
-    "tfgpu_resident_stats", "tfgpu_resident_fetch", "tfgpu_result_rows_in", "tfgpu_result_rows_out",
-    "tfgpu_result_n_errors", "tfgpu_result_errors", "tfgpu_result_batch", "tfgpu_result_bytes",
-    "tfgpu_result_bytes_len", "tfgpu_result_raw_len", "tfgpu_result_n_frames", "tfgpu_result_release",
-    "tfgpu_engine_launch_count", "tfgpu_profile_enable", "tfgpu_profile_read",
-    "tfgpu_deflate_stream_open", "tfgpu_deflate_stream_append", "tfgpu_deflate_stream_close", "tfgpu_deflate_stream_free",
-]
+EXPORTED_SYMBOLS = list(abi.TFGPU_H_PROTOTYPES)     # the functions of include/tfgpu.h
 
 
 class DeflateStream:
@@ -136,46 +91,28 @@ class DeflateStream:
 
 def debezium_table_schema(schema_text: str):
     """The table schema the reference derives from a Kafka Connect envelope schema's `after` struct with the default receivers
-    (pkg/debezium/receiver.go:46-62, receiver_engine.go:104-141, common/field_receiver_default.go:15-30): key = !optional."""
-    sch = json.loads(schema_text)
-    node = next((f for f in sch.get("fields", []) if f.get("field") == "after"), None)
-    if node is None:
-        raise EngineError(-1, "debezium schema has no 'after' struct")
-    out = []
-    for f in node.get("fields", []):
-        kt, nm = f.get("type"), f.get("name", "")
-        if kt in ("int8", "int16", "int32", "int64", "boolean"): yt = kt
-        elif kt == "string": yt = "utf8"
-        elif kt in ("float", "double"): yt = "double"
-        elif kt == "bytes": yt = "utf8" if nm == "org.apache.kafka.connect.data.Decimal" else "string"
-        elif kt == "struct" and nm == "io.debezium.data.geometry.Point": yt = "utf8"
-        elif kt == "struct" and nm == "io.debezium.data.VariableScaleDecimal": yt = "double"
-        else: raise EngineError(-1, f"debezium: kafka type {kt} / {nm} has no default receiver on the device")
-        out.append({"name": f["field"], "type": yt, "key": not f.get("optional", False)})
-    return out
+    (pkg/debezium/receiver.go:46-62, receiver_engine.go:104-141, common/field_receiver_default.go:15-30): [{"name", "type", "key"}] of
+    debezium_schema_validate, key = !optional; EngineError for a schema tfgpu_parse_debezium refuses."""
+    return [{k: f[k] for k in ("name", "type", "key")} for f in debezium_schema_validate(schema_text)]
+
+
+def _queue_batches(fn: str, sizes, *limits):
+    """A host-only queue batcher over per-row sizes: first row of every message, then n."""
+    a = np.asarray(sizes, dtype=np.uint32); st = np.zeros(len(a) + 1, dtype=np.uint64); k = C.c_uint64()
+    rc = getattr(load_library(), fn)(a.ctypes.data, len(a), *limits, st.ctypes.data, len(st), C.byref(k))
+    if rc != 0:
+        raise EngineError(rc, fn)
+    return [int(x) for x in st[:k.value + 1]]
 
 
 def queue_debezium_batches(value_sizes, max_message_size: int = 0):
     """MergeWithMaxMessageSize of the queue Debezium serializer (host only): first row of every merged message, then n."""
-    import numpy as np
-    L = load_library()
-    a = np.asarray(value_sizes, dtype=np.uint32); st = np.zeros(len(a) + 1, dtype=np.uint64); k = C.c_uint64()
-    L.tfgpu_queue_debezium_batches.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
-    rc = L.tfgpu_queue_debezium_batches(a.ctypes.data, len(a), max_message_size, st.ctypes.data, len(st), C.byref(k))
-    if rc != 0:
-        raise EngineError(rc, "tfgpu_queue_debezium_batches")
-    return [int(x) for x in st[:k.value + 1]]
+    return _queue_batches("tfgpu_queue_debezium_batches", value_sizes, max_message_size)
 
 
 def queue_json_batches(json_row_sizes, max_message_size: int = 0, max_change_items: int = 0):
     """BatchJSON of the queue JSON serializer (host only): first row of every message, then n."""
-    import numpy as np
-    L = load_library()
-    a = np.asarray(json_row_sizes, dtype=np.uint32); st = np.zeros(len(a) + 1, dtype=np.uint64); k = C.c_uint64()
-    rc = L.tfgpu_queue_json_batches(a.ctypes.data, len(a), max_message_size, max_change_items, st.ctypes.data, len(st), C.byref(k))
-    if rc != 0:
-        raise EngineError(rc, "tfgpu_queue_json_batches")
-    return [int(x) for x in st[:k.value + 1]]
+    return _queue_batches("tfgpu_queue_json_batches", json_row_sizes, max_message_size, max_change_items)
 
 
 def json_result_schema(fields, opts: Optional[dict] = None):
@@ -198,40 +135,31 @@ def json_result_schema(fields, opts: Optional[dict] = None):
     return out
 
 
-def debezium_schema_validate(schema_text: str) -> list:
-    """Host-only: [{"name","type","key","recv","scale"}] the C++ side derives from an envelope schema (no GPU needed), or raises EngineError."""
-    L = load_library()
-    out = C.create_string_buffer(1 << 20); err = C.create_string_buffer(4096)
-    L.tfgpu_debezium_schema_validate.argtypes = [C.c_char_p, C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64]
-    rc = L.tfgpu_debezium_schema_validate(schema_text.encode(), out, len(out), err, len(err))
+def _describe(fn: str, cap: int, *args):
+    """A host-only *_validate call with a `cap`-byte describe buffer (too small a buffer is an error, not a truncation): its JSON, or
+    EngineError with the call's message."""
+    out = C.create_string_buffer(cap); err = C.create_string_buffer(4096)
+    rc = getattr(load_library(), fn)(*args, out, len(out), err, len(err))
     if rc != 0:
         raise EngineError(rc, err.value.decode(errors="replace"))
     return json.loads(out.value.decode())
+
+
+def debezium_schema_validate(schema_text: str) -> list:
+    """Host-only: [{"name","type","key","recv","scale"}] the C++ side derives from an envelope schema (no GPU needed), or raises EngineError."""
+    return _describe("tfgpu_debezium_schema_validate", 1 << 20, schema_text.encode())
 
 
 def emit_debezium_validate(namespace: str, name: str, schema, transformers, opts: dict) -> dict:
     """Host-only set-up of the Debezium emitter (no GPU needed): {"forms", "keys", "template"} or raises EngineError."""
-    L = load_library()
-    sj = schema if isinstance(schema, str) else json.dumps([{k: v for k, v in c.items() if not k.startswith("_")} for c in schema])
-    out = C.create_string_buffer(1 << 22); err = C.create_string_buffer(4096)
-    L.tfgpu_emit_debezium_validate.argtypes = [C.c_char_p] * 5 + [C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64]
-    rc = L.tfgpu_emit_debezium_validate(namespace.encode(), name.encode(), sj.encode(), json.dumps(transformers or []).encode(), json.dumps(opts).encode(),
-                                        out, len(out), err, len(err))
-    if rc != 0:
-        raise EngineError(rc, err.value.decode(errors="replace"))
-    return json.loads(out.value.decode())
+    return _describe("tfgpu_emit_debezium_validate", 1 << 22, namespace.encode(), name.encode(), abi.schema_json(schema).encode(),
+                     json.dumps(transformers or []).encode(), json.dumps(opts).encode())
 
 
 def plan_validate(namespace: str, name: str, schema, transformers=None, sink=None) -> dict:
     """Host-only plan construction (no GPU needed): returns the describe JSON or raises EngineError."""
-    L = load_library()
-    sj = schema if isinstance(schema, str) else json.dumps([{k: v for k, v in c.items() if not k.startswith("_")} for c in schema])
-    out = C.create_string_buffer(1 << 20); err = C.create_string_buffer(4096)
-    rc = L.tfgpu_plan_validate(namespace.encode(), name.encode(), sj.encode(), json.dumps(transformers or []).encode(),
-                               None if sink is None else json.dumps(sink).encode(), out, len(out), err, len(err))
-    if rc != 0:
-        raise EngineError(rc, err.value.decode(errors="replace"))
-    return json.loads(out.value.decode())
+    return _describe("tfgpu_plan_validate", 1 << 20, namespace.encode(), name.encode(), abi.schema_json(schema).encode(),
+                     json.dumps(transformers or []).encode(), None if sink is None else json.dumps(sink).encode())
 
 
 @dataclass
@@ -240,8 +168,36 @@ class PushResult:
     rows_out: int
     raw_len: int
     n_frames: int
-    wire: bytes
+    wire: bytes                            # empty with copy_bytes=False: the bytes stay in the engine's pinned landing buffer
     errors: List[Tuple[int, int, int]]     # (input row, TF_ROWERR_*, transformer index)
+    wire_len: Optional[int] = None
+    row_sizes: Any = None                  # push_encode: list of int (row-text formats); emit_debezium: numpy uint32
+    key_sizes: Any = None                  # emit_debezium: numpy uint32 per row
+    msg_sizes: Any = None                  # emit_debezium: numpy uint32 (rows_out x 7)
+    part_ids: Any = None                   # push_encode with a sharder: numpy uint32 per row
+
+
+def _row_errors(L, res) -> List[Tuple[int, int, int]]:
+    ep = L.tfgpu_result_errors(res)
+    return [(ep[k].row, ep[k].code, ep[k].term) for k in range(L.tfgpu_result_n_errors(res))]
+
+
+def _push_result(L, res, copy_bytes: bool, **per_row) -> PushResult:
+    """PushResult of a wire-format result; per_row: the per-row arrays of the call that made it."""
+    n = L.tfgpu_result_bytes_len(res)
+    return PushResult(L.tfgpu_result_rows_in(res), L.tfgpu_result_rows_out(res), L.tfgpu_result_raw_len(res), L.tfgpu_result_n_frames(res),
+                      C.string_at(L.tfgpu_result_bytes(res), n) if (copy_bytes and n) else b"", _row_errors(L, res), n, **per_row)
+
+
+def _u32s(p, *shape):
+    """Copy of a uint32 array of the result (empty without rows or when NULL)."""
+    return np.ctypeslib.as_array(p, shape=shape).copy() if (p and shape[0]) else np.zeros((0,) + shape[1:], np.uint32)
+
+
+def _part_ids(L, res, rows_out):
+    """sharder_transformer: ChangeItem.PartID of every output row as an integer (numpy uint32), None without a sharder."""
+    pp = L.tfgpu_result_part_ids(res)
+    return _u32s(pp, rows_out) if (pp and rows_out) else None
 
 
 class Engine:
@@ -276,11 +232,10 @@ class Engine:
         self._check(self._L.tfgpu_engine_set_stream(self._h, C.c_void_p(cuda_stream_ptr or 0)))
 
     def plan(self, namespace: str, name: str, schema, transformers=None, sink=None) -> int:
-        sj = schema if isinstance(schema, str) else json.dumps([{k: v for k, v in c.items() if not k.startswith("_")} for c in schema])
         tj = json.dumps(transformers or [])
         kj = None if sink is None else json.dumps(sink).encode()
         pid = C.c_int(-1)
-        self._check(self._L.tfgpu_plan(self._h, namespace.encode(), name.encode(), sj.encode(), tj.encode(), kj, C.byref(pid)))
+        self._check(self._L.tfgpu_plan(self._h, namespace.encode(), name.encode(), abi.schema_json(schema).encode(), tj.encode(), kj, C.byref(pid)))
         return pid.value
 
     def describe(self, plan_id: int) -> dict:
@@ -298,32 +253,15 @@ class Engine:
             self._check(self._L.tfgpu_push_encode_selective(self._h, plan_id, wire_fmt, C.byref(tb), int(selective), C.byref(res)))
         try:
             L = self._L
-            n = L.tfgpu_result_bytes_len(res)
-            wire = C.string_at(L.tfgpu_result_bytes(res), n) if (copy_bytes and n) else b""
-            ne = L.tfgpu_result_n_errors(res)
-            ep = L.tfgpu_result_errors(res)
-            errs = [(ep[k].row, ep[k].code, ep[k].term) for k in range(ne)]
-            out = PushResult(L.tfgpu_result_rows_in(res), L.tfgpu_result_rows_out(res), L.tfgpu_result_raw_len(res),
-                             L.tfgpu_result_n_frames(res), wire, errs)
-            out.wire_len = n
-            rs = L.tfgpu_result_row_sizes(res)
-            out.row_sizes = [int(rs[k]) for k in range(out.rows_out)] if rs else None
-            out.part_ids = self._part_ids(res, out.rows_out)
-            return out
+            nout, rs = L.tfgpu_result_rows_out(res), L.tfgpu_result_row_sizes(res)
+            return _push_result(L, res, copy_bytes, row_sizes=_u32s(rs, nout).tolist() if rs else None, part_ids=_part_ids(L, res, nout))
         finally:
             self._L.tfgpu_result_release(res)
 
     def h2d_bytes(self) -> int:
         return int(self._L.tfgpu_engine_h2d_bytes(self._h))
 
-    def _part_ids(self, res, rows_out):
-        """sharder_transformer: ChangeItem.PartID of every output row as an integer (numpy uint32), None without a sharder."""
-        import numpy as np
-        pp = self._L.tfgpu_result_part_ids(res)
-        return np.ctypeslib.as_array(pp, shape=(int(rows_out),)).copy() if (pp and rows_out) else None
-
     def _result_batch(self, res):
-        import numpy as np
         L = self._L
         ob = L.tfgpu_result_batch(res)
         n = int(L.tfgpu_result_rows_out(res))
@@ -344,11 +282,8 @@ class Engine:
                     dt = abi.FIXED_DTYPE[t]
                     cols.append(abi.Column(t, values=arr(c.values, n * np.dtype(dt).itemsize, dt), validity=arr(c.validity, (n + 7) // 8, np.uint8),
                                            aux=arr(c.aux, 4 * n, np.uint32)))
-        ne = L.tfgpu_result_n_errors(res); ep = L.tfgpu_result_errors(res)
-        errs = [(ep[k].row, ep[k].code, ep[k].term) for k in range(ne)]
-        out = abi.Batch(n, cols)
-        self.last_part_ids = self._part_ids(res, n)       # of the batch just returned (push_columns / parsers)
-        return out, errs
+        self.last_part_ids = _part_ids(L, res, n)       # of the batch just returned (push_columns / parsers)
+        return abi.Batch(n, cols), _row_errors(L, res)
 
     def push_columns(self, plan_id: int, batch: abi.Batch) -> Tuple[abi.Batch, List[Tuple[int, int, int]]]:
         """Transformer chain only: (Transformed rows as a host Batch, row errors) — abstract.TransformerResult."""
@@ -374,20 +309,13 @@ class Engine:
         wire bytes in the engine's pinned landing buffer and only reports their length."""
         ptr, total, keep = self._host_bytes(data)
         res = C.c_void_p()
-        self._L.tfgpu_parse_csv.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_void_p]
-        self._check(self._L.tfgpu_parse_csv(self._h, plan_id, json.dumps(opts or {}).encode(), ptr, total, abi.TF_MEM_HOST, wire_fmt, C.cast(C.pointer(res), C.c_void_p)))
+        self._check(self._L.tfgpu_parse_csv(self._h, plan_id, json.dumps(opts or {}).encode(), ptr, total, abi.TF_MEM_HOST, wire_fmt, C.byref(res)))
         try:
-            L = self._L
-            consumed = int(L.tfgpu_result_consumed(res))
+            consumed = int(self._L.tfgpu_result_consumed(res))
             if wire_fmt == 0:
                 b, errs = self._result_batch(res)
                 return b, errs, consumed
-            n = L.tfgpu_result_bytes_len(res)
-            ne = L.tfgpu_result_n_errors(res); ep = L.tfgpu_result_errors(res)
-            out = PushResult(L.tfgpu_result_rows_in(res), L.tfgpu_result_rows_out(res), L.tfgpu_result_raw_len(res), L.tfgpu_result_n_frames(res),
-                             C.string_at(L.tfgpu_result_bytes(res), n) if (n and copy_bytes) else b"", [(ep[k].row, ep[k].code, ep[k].term) for k in range(ne)])
-            out.wire_len = n
-            return out, consumed
+            return _push_result(self._L, res, copy_bytes), consumed
         finally:
             self._L.tfgpu_result_release(res)
 
@@ -396,13 +324,11 @@ class Engine:
         """Debezium messages -> typed columns (default receivers) -> the plan's chain, on the device; one row per message.
         wire_fmt 0: (Batch, row errors, meta) with meta = {"selection", "kinds", "tx_id", "lsn", "commit_time"} (numpy; the last four
         per MESSAGE, selection per output row); otherwise (PushResult, meta)."""
-        import numpy as np
         ends = np.asarray(msg_ends, dtype=np.uint64)
         opts = {"schema_text": schema_text, "schema_registry": schema_registry, "schema_id": schema_id, "check_table": check_table}
         ptr, total, keep = self._host_bytes(data)
         res = C.c_void_p()
-        self._L.tfgpu_parse_debezium.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p]
-        self._check(self._L.tfgpu_parse_debezium(self._h, plan_id, json.dumps(opts).encode(), ptr, total, abi.TF_MEM_HOST, ends.ctypes.data, len(ends), wire_fmt, C.cast(C.pointer(res), C.c_void_p)))
+        self._check(self._L.tfgpu_parse_debezium(self._h, plan_id, json.dumps(opts).encode(), ptr, total, abi.TF_MEM_HOST, ends.ctypes.data, len(ends), wire_fmt, C.byref(res)))
         try:
             L = self._L
             nin, nout = int(L.tfgpu_result_rows_in(res)), int(L.tfgpu_result_rows_out(res))
@@ -414,11 +340,7 @@ class Engine:
             if wire_fmt == 0:
                 b, errs = self._result_batch(res)
                 return b, errs, meta
-            nb = L.tfgpu_result_bytes_len(res); ne = L.tfgpu_result_n_errors(res); ep = L.tfgpu_result_errors(res)
-            out = PushResult(nin, nout, L.tfgpu_result_raw_len(res), L.tfgpu_result_n_frames(res), C.string_at(L.tfgpu_result_bytes(res), nb) if (nb and copy_bytes) else b"",
-                             [(ep[k].row, ep[k].code, ep[k].term) for k in range(ne)])
-            out.wire_len = nb
-            return out, meta
+            return _push_result(L, res, copy_bytes), meta
         finally:
             self._L.tfgpu_result_release(res)
 
@@ -435,37 +357,23 @@ class Engine:
         `key_sizes` / `row_sizes` give the first key and the total per row, `msg_sizes` (rows_out x 7) the message count and
         (key bytes, value bytes | 0xFFFFFFFF) per message. meta: {"id", "lsn", "commit_time", "txid_offsets", "txid_heap"} arrays in the
         memory space of the batch. old / old_present / old_row_has: ChangeItem.OldKeys (tf_old_keys)."""
-        import numpy as np
         tb = batch.as_struct()
         meta = meta or {}
         m, keep = abi.make_row_meta(meta.get("id"), meta.get("lsn"), meta.get("commit_time"), meta.get("txid_offsets"), meta.get("txid_heap"))
         res = C.c_void_p()
         ok, okeep = (abi.make_old_keys(old, old_present or [], old_row_has) if old is not None else (None, None))
-        self._L.tfgpu_emit_debezium_crud.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        self._check(self._L.tfgpu_emit_debezium_crud(self._h, plan_id, json.dumps(opts).encode(), C.cast(C.pointer(tb), C.c_void_p),
-                                                     C.cast(C.pointer(ok), C.c_void_p) if ok is not None else None, C.cast(C.pointer(m), C.c_void_p), C.cast(C.pointer(res), C.c_void_p)))
+        self._check(self._L.tfgpu_emit_debezium_crud(self._h, plan_id, json.dumps(opts).encode(), C.byref(tb), C.byref(ok) if ok is not None else None,
+                                                     C.byref(m), C.byref(res)))
         try:
             L = self._L
-            n = L.tfgpu_result_bytes_len(res)
-            wire = C.string_at(L.tfgpu_result_bytes(res), n) if (copy_bytes and n) else b""
-            ne = L.tfgpu_result_n_errors(res); ep = L.tfgpu_result_errors(res)
-            out = PushResult(L.tfgpu_result_rows_in(res), L.tfgpu_result_rows_out(res), L.tfgpu_result_raw_len(res), 0, wire,
-                             [(ep[k].row, ep[k].code, ep[k].term) for k in range(ne)])
-            out.wire_len = n
-            k = int(out.rows_out)
-            rs = L.tfgpu_result_row_sizes(res); ks = L.tfgpu_result_key_sizes(res)
-            out.row_sizes = np.ctypeslib.as_array(rs, shape=(k,)).copy() if (rs and k) else np.zeros(0, np.uint32)
-            out.key_sizes = np.ctypeslib.as_array(ks, shape=(k,)).copy() if (ks and k) else np.zeros(0, np.uint32)
-            L.tfgpu_result_dbz_msg_sizes.restype = C.POINTER(C.c_uint32); L.tfgpu_result_dbz_msg_sizes.argtypes = [C.c_void_p]
-            ms = L.tfgpu_result_dbz_msg_sizes(res)
-            out.msg_sizes = np.ctypeslib.as_array(ms, shape=(k, 7)).copy() if (ms and k) else np.zeros((0, 7), np.uint32)
-            return out
+            k = L.tfgpu_result_rows_out(res)
+            return _push_result(L, res, copy_bytes, row_sizes=_u32s(L.tfgpu_result_row_sizes(res), k), key_sizes=_u32s(L.tfgpu_result_key_sizes(res), k),
+                                msg_sizes=_u32s(L.tfgpu_result_dbz_msg_sizes(res), k, 7))
         finally:
             self._L.tfgpu_result_release(res)
 
     def measure(self, batch: abi.Batch):
         """Measurer middleware: ChangeItem.Size.Values of every row (numpy uint64) and their sum."""
-        import numpy as np
         tb = batch.as_struct(); per = np.zeros(batch.nrows, dtype=np.uint64); tot = C.c_uint64()
         self._check(self._L.tfgpu_measure(self._h, C.byref(tb), per.ctypes.data, C.byref(tot)))
         return per, tot.value
@@ -475,30 +383,18 @@ class Engine:
         msgs: [(end, offset, write_sec, write_nsec)] (default: one message = all of `data`).
         wire_fmt 0: (Batch, row errors, non-empty lines); otherwise PushResult (copy_bytes=False leaves the wire bytes in the
         engine's pinned landing buffer and only reports their length)."""
-        tensor = hasattr(data, "data_ptr")                  # a (pinned) torch uint8 tensor: its storage is used in place
-        total = int(data.numel()) if tensor else len(data)
+        ptr, total, keep = self._host_bytes(data)
         msgs = msgs if msgs is not None else [(total, 0, 0, 0)]
         ms = (abi.TfMsg * max(1, len(msgs)))()
         for k, (end, off, ws, wn) in enumerate(msgs):
             ms[k].end, ms[k].offset, ms[k].write_sec, ms[k].write_nsec = end, off, ws, wn
-        if tensor:
-            ptr = C.c_void_p(data.data_ptr())
-        else:
-            buf = C.c_char_p(data if data else b"\0")      # the bytes object's own storage: no copy
-            ptr = C.cast(buf, C.c_void_p)
         res = C.c_void_p()
         self._check(self._L.tfgpu_parse_json(self._h, plan_id, json.dumps(opts or {}).encode(), ptr, total, abi.TF_MEM_HOST, ms, len(msgs), wire_fmt, C.byref(res)))
         try:
-            L = self._L
             if wire_fmt == 0:
                 b, errs = self._result_batch(res)
-                return b, errs, int(L.tfgpu_result_rows_in(res))
-            n = L.tfgpu_result_bytes_len(res)
-            ne = L.tfgpu_result_n_errors(res); ep = L.tfgpu_result_errors(res)
-            out = PushResult(L.tfgpu_result_rows_in(res), L.tfgpu_result_rows_out(res), L.tfgpu_result_raw_len(res), L.tfgpu_result_n_frames(res),
-                             C.string_at(L.tfgpu_result_bytes(res), n) if (n and copy_bytes) else b"", [(ep[k].row, ep[k].code, ep[k].term) for k in range(ne)])
-            out.wire_len = n
-            return out
+                return b, errs, int(self._L.tfgpu_result_rows_in(res))
+            return _push_result(self._L, res, copy_bytes)
         finally:
             self._L.tfgpu_result_release(res)
 

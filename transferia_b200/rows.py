@@ -5,7 +5,6 @@ helpers below (`go.int32(5)`, `go.string("x")`, `go.time(sec, nsec)`), because P
 from __future__ import annotations
 
 import ctypes as C
-import json
 import struct
 from dataclasses import dataclass, field
 from typing import Any, Dict, List, Optional, Sequence, Tuple
@@ -13,6 +12,7 @@ from typing import Any, Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import abi, engine
+from .abi import TfItem, TfRows, TfTable
 
 # kinds (kind.go:5-43)
 KIND_INSERT, KIND_UPDATE, KIND_DELETE = 0, 1, 2
@@ -68,21 +68,6 @@ class ChangeItem:
     txid: bytes = b""; part_id: bytes = b""
 
 
-class TfTable(C.Structure):
-    _fields_ = [("schema", C.c_char_p), ("table", C.c_char_p), ("schema_json", C.c_char_p)]
-
-
-class TfItem(C.Structure):
-    _fields_ = [("lsn", C.c_uint64), ("commit_time", C.c_uint64), ("size_read", C.c_uint64), ("size_values", C.c_uint64), ("values_off", C.c_uint64), ("old_keys_off", C.c_uint64),
-                ("id", C.c_uint32), ("table", C.c_uint32), ("n_values", C.c_uint32), ("txid_off", C.c_uint32), ("txid_len", C.c_uint32),
-                ("part_off", C.c_uint32), ("part_len", C.c_uint32), ("counter", C.c_int32), ("kind", C.c_uint8), ("flags", C.c_uint8), ("pad", C.c_uint8 * 2)]
-
-
-class TfRows(C.Structure):
-    _fields_ = [("n_items", C.c_uint64), ("items", C.POINTER(TfItem)), ("n_tables", C.c_uint32), ("pad", C.c_uint32), ("tables", C.POINTER(TfTable)),
-                ("values", C.c_void_p), ("values_len", C.c_uint64), ("strings", C.c_void_p), ("strings_len", C.c_uint64)]
-
-
 NO_OLD_KEYS = (1 << 64) - 1
 
 
@@ -119,8 +104,7 @@ class RowsImage:
         self._tabs = (TfTable * max(1, len(tables)))()
         self._keep = []
         for k, (ns, name, schema) in enumerate(tables):
-            sj = (None if schema is None else json.dumps([{k: v for k, v in c.items() if not k.startswith("_")} for c in schema]).encode() if not isinstance(schema, (bytes, str))
-                  else (schema.encode() if isinstance(schema, str) else schema))
+            sj = None if schema is None else schema if isinstance(schema, bytes) else abi.schema_json(schema).encode()
             self._keep.append((ns.encode(), name.encode(), sj))
             self._tabs[k].schema, self._tabs[k].table, self._tabs[k].schema_json = self._keep[-1]
         r = TfRows()
@@ -181,25 +165,6 @@ def batch_from_struct(tb: abi.TfBatch) -> abi.Batch:
     return abi.Batch(n, cols, _view(tb.kinds, n), abi.TF_MEM_HOST)
 
 
-_bound = False
-
-
-def _lib():
-    global _bound
-    L = engine.load_library()
-    if not _bound:
-        vp, u64 = C.c_void_p, C.c_uint64
-        L.tfgpu_columnar_create.argtypes = [C.POINTER(vp)]
-        L.tfgpu_columnar_destroy.argtypes = [vp]
-        L.tfgpu_columnar_last_error.argtypes = [vp]; L.tfgpu_columnar_last_error.restype = C.c_char_p
-        L.tfgpu_rows_to_batch.argtypes = [vp, C.POINTER(TfRows), C.c_uint32, vp, u64, C.c_int, C.POINTER(C.POINTER(abi.TfBatch)),
-                                          C.POINTER(C.POINTER(abi.TfRowMeta)), C.POINTER(C.POINTER(abi.TfOldKeys))]
-        L.tfgpu_batch_to_rows.argtypes = [C.POINTER(abi.TfBatch), vp, u64, vp, C.POINTER(u64)]
-        L.tfgpu_batch_gather.argtypes = [vp, C.POINTER(abi.TfBatch), vp, C.c_int, C.POINTER(C.POINTER(abi.TfBatch)), C.POINTER(C.POINTER(C.c_uint32))]
-        _bound = True
-    return L
-
-
 @dataclass
 class Transposed:
     batch: abi.Batch
@@ -214,7 +179,7 @@ class Columnar:
     """Pooled column buffers + the transposer (tfgpu_columnar)."""
 
     def __init__(self):
-        self._L = _lib(); self._h = C.c_void_p()
+        self._L = engine.load_library(); self._h = C.c_void_p()
         rc = self._L.tfgpu_columnar_create(C.byref(self._h))
         if rc: raise engine.EngineError(rc, "tfgpu_columnar_create")
 
@@ -250,7 +215,7 @@ class Columnar:
 
 def batch_to_rows(batch: abi.Batch) -> Tuple[bytes, np.ndarray]:
     """tfgpu_batch_to_rows: (value images back to back, nrows + 1 offsets)."""
-    L = _lib(); tb = batch.as_struct()
+    L = engine.load_library(); tb = batch.as_struct()
     off = np.zeros(batch.nrows + 1, dtype=np.uint64); need = C.c_uint64()
     L.tfgpu_batch_to_rows(C.byref(tb), None, 0, off.ctypes.data, C.byref(need))
     out = np.zeros(int(need.value) + 1, dtype=np.uint8)

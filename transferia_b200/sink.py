@@ -13,45 +13,16 @@ from typing import List, Optional, Tuple
 
 import numpy as np
 
-from . import engine
+from . import abi, engine
+from .abi import TF_SINK_FN, TfSinkEvent, TfSinkStats  # noqa: F401  (TfSinkEvent: the struct a callback receives)
 
-SINK_SYMBOLS = [
-    "tfgpu_ch_open", "tfgpu_ch_close", "tfgpu_ch_last_error", "tfgpu_ch_server_info", "tfgpu_ch_exception_code",
-    "tfgpu_ch_insert_begin", "tfgpu_ch_insert_columns", "tfgpu_ch_insert_data", "tfgpu_ch_insert_end", "tfgpu_ch_stats",
-    "tfgpu_ch_insert_query", "tfgpu_host_cityhash128", "tfgpu_regex_replace_all",
-    "tfgpu_columnar_create", "tfgpu_columnar_destroy", "tfgpu_columnar_last_error", "tfgpu_rows_to_batch", "tfgpu_batch_to_rows", "tfgpu_batch_gather", "tfgpu_batch_gather_sel",
-]
-
-_bound = False
-
-
-def lib():
-    global _bound
-    L = engine.load_library()
-    if _bound:
-        return L
-    vp, cp, i, u64 = C.c_void_p, C.c_char_p, C.c_int, C.c_uint64
-    L.tfgpu_ch_open.argtypes = [i, cp, C.POINTER(vp)]
-    L.tfgpu_ch_close.argtypes = [vp]
-    L.tfgpu_ch_last_error.argtypes = [vp]; L.tfgpu_ch_last_error.restype = cp
-    L.tfgpu_ch_server_info.argtypes = [vp]; L.tfgpu_ch_server_info.restype = cp
-    L.tfgpu_ch_exception_code.argtypes = [vp]
-    L.tfgpu_ch_insert_begin.argtypes = [vp, cp, cp, cp]
-    L.tfgpu_ch_insert_columns.argtypes = [vp]; L.tfgpu_ch_insert_columns.restype = cp
-    L.tfgpu_ch_insert_data.argtypes = [vp, vp, u64]
-    L.tfgpu_ch_insert_end.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
-    L.tfgpu_ch_stats.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
-    L.tfgpu_ch_insert_query.argtypes = [cp, cp, cp, i, C.c_char_p, u64]; L.tfgpu_ch_insert_query.restype = C.c_int64
-    L.tfgpu_host_cityhash128.argtypes = [vp, u64, C.POINTER(u64)]; L.tfgpu_host_cityhash128.restype = None
-    L.tfgpu_regex_replace_all.argtypes = [cp, cp, cp, u64, cp, u64]; L.tfgpu_regex_replace_all.restype = C.c_int64
-    _bound = True
-    return L
+SINK_SYMBOLS = list(abi.TFGPU_SINK_H_PROTOTYPES)    # the functions of include/tfgpu_sink.h
 
 
 def host_cityhash128(data: bytes) -> Tuple[int, int]:
     out = (C.c_uint64 * 2)()
     buf = C.create_string_buffer(data, len(data)) if data else None
-    lib().tfgpu_host_cityhash128(C.cast(buf, C.c_void_p) if buf else None, len(data), out)
+    engine.load_library().tfgpu_host_cityhash128(C.cast(buf, C.c_void_p) if buf else None, len(data), out)
     return int(out[0]), int(out[1])
 
 
@@ -64,7 +35,7 @@ def regex_replace_all(pattern: str, rule: str, src: bytes) -> bytes:
     cap = max(64, 2 * len(src) + 64)
     while True:
         out = C.create_string_buffer(cap)
-        n = lib().tfgpu_regex_replace_all(pat, rl, src, len(src), out, cap)
+        n = engine.load_library().tfgpu_regex_replace_all(pat, rl, src, len(src), out, cap)
         if n < 0:
             raise engine.EngineError(int(n), "tfgpu_regex_replace_all")
         if n <= cap:
@@ -75,7 +46,7 @@ def regex_replace_all(pattern: str, rule: str, src: bytes) -> bytes:
 def insert_query(database: str, table: str, columns: List[str], updateable: bool = False) -> str:
     """doOperation's statement (sink_table.go:633-660) as clickhouse-go sends it (cut at VALUES)."""
     out = C.create_string_buffer(1 << 16)
-    n = lib().tfgpu_ch_insert_query(database.encode(), table.encode(), json.dumps(columns).encode(), int(updateable), out, len(out))
+    n = engine.load_library().tfgpu_ch_insert_query(database.encode(), table.encode(), json.dumps(columns).encode(), int(updateable), out, len(out))
     if n < 0:
         raise engine.EngineError(int(n), "tfgpu_ch_insert_query")
     return out.raw[:n].decode()
@@ -85,7 +56,7 @@ class ClickHouseWriter:
     """One native-protocol connection over a connected socket (the caller dials and keeps the socket object alive)."""
 
     def __init__(self, sock, database="default", user="default", password="", compression=True, read_timeout_ms=300000, client_name=None):
-        self._L = lib()
+        self._L = engine.load_library()
         self._sock = sock
         self._h = C.c_void_p()
         opts = {"database": database, "user": user, "password": password, "compression": compression, "read_timeout_ms": read_timeout_ms}
@@ -138,25 +109,7 @@ class ClickHouseWriter:
 
 
 # ------------------------------------------------------------------ Sinker.Push as one call (tfgpu_sink_*)
-SINK_SYMBOLS += ["tfgpu_sink_create", "tfgpu_sink_destroy", "tfgpu_sink_last_error", "tfgpu_sink_set_callback", "tfgpu_sink_set_clickhouse",
-                 "tfgpu_sink_push", "tfgpu_sink_stats",
-                 "tfgpu_dispatcher_create", "tfgpu_dispatcher_submit", "tfgpu_dispatcher_wait", "tfgpu_dispatcher_drain", "tfgpu_dispatcher_destroy"]
 EV_ROWS, EV_ITEM, EV_ERRORS = 1, 2, 3
-
-
-class TfSinkEvent(C.Structure):
-    _fields_ = [("type", C.c_int32), ("table", C.c_uint32), ("out_schema", C.c_char_p), ("out_table", C.c_char_p), ("n_items", C.c_uint64),
-                ("item_idx", C.POINTER(C.c_uint64)), ("errors", C.c_void_p), ("batch", C.c_void_p), ("wire", C.c_void_p),
-                ("wire_len", C.c_uint64), ("raw_len", C.c_uint64), ("n_frames", C.c_uint64), ("msg_sizes", C.POINTER(C.c_uint32)), ("plan_id", C.c_int32), ("pad", C.c_int32)]
-
-
-class TfSinkStats(C.Structure):
-    _fields_ = [(n, C.c_uint64) for n in ("pushes", "downstream_pushes", "change_items_pushed", "row_events_pushed", "inflight_bytes", "filter_dropped",
-                                          "transform_dropped", "transform_errors", "max_commit_time", "min_commit_time", "without_commit_time", "wire_bytes",
-                                          "metering_input_rows", "metering_output_rows")]
-
-
-_SINK_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(TfSinkEvent))
 
 
 class Sink:
@@ -169,21 +122,13 @@ class Sink:
                  record: str = "full"):
         """record: "full" keeps item indexes and copies of the delivered columns per event (tests); "counts" keeps type / table / n_items
         only (timing runs: the copies would be what is measured)."""
-        from . import abi, rows as _rows
-        self._L = lib()
-        vp = C.c_void_p
-        self._L.tfgpu_sink_create.argtypes = [vp, C.c_char_p, C.POINTER(vp)]
-        self._L.tfgpu_sink_destroy.argtypes = [vp]
-        self._L.tfgpu_sink_last_error.argtypes = [vp]; self._L.tfgpu_sink_last_error.restype = C.c_char_p
-        self._L.tfgpu_sink_set_callback.argtypes = [vp, _SINK_FN, vp]
-        self._L.tfgpu_sink_set_clickhouse.argtypes = [vp, vp]
-        self._L.tfgpu_sink_push.argtypes = [vp, vp]
-        self._L.tfgpu_sink_stats.argtypes = [vp, C.POINTER(TfSinkStats)]
+        from . import rows as _rows
+        self._L = engine.load_library()
         cfg = {"transformers": transformers or [], "wire_fmt": wire_fmt, "system_tables": list(system_tables), "exclude_system_tables": exclude_system_tables,
                "errors_output": errors_output, "database": database, "updateable": updateable}
         if debezium is not None:
             cfg["debezium"] = debezium
-        self._h = vp()
+        self._h = C.c_void_p()
         rc = self._L.tfgpu_sink_create(eng._h if eng is not None else None, json.dumps(cfg).encode(), C.byref(self._h))
         if rc:
             raise engine.EngineError(rc, "tfgpu_sink_create")
@@ -215,7 +160,7 @@ class Sink:
                 d["errors"] = [(errs[k].row, errs[k].code, errs[k].term) for k in range(ev.n_items)]
             self.events.append(d)
             return int(self._downstream(d)) if self._downstream else 0
-        self._cb = _SINK_FN(_cb)
+        self._cb = TF_SINK_FN(_cb)
         self._L.tfgpu_sink_set_callback(self._h, self._cb, None)
         if clickhouse is not None:
             rc = self._L.tfgpu_sink_set_clickhouse(self._h, clickhouse._h)
@@ -251,12 +196,7 @@ class Dispatcher:
     deliveries in submission order (SURVEY §8e). submit() returns a sequence number; wait(seq) the outcome of that batch's push."""
 
     def __init__(self, sinks):
-        self._L = lib(); vp = C.c_void_p
-        self._L.tfgpu_dispatcher_create.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(vp)]
-        self._L.tfgpu_dispatcher_submit.argtypes = [vp, vp, C.POINTER(C.c_uint64)]
-        self._L.tfgpu_dispatcher_wait.argtypes = [vp, C.c_uint64]
-        self._L.tfgpu_dispatcher_drain.argtypes = [vp]
-        self._L.tfgpu_dispatcher_destroy.argtypes = [vp]
+        self._L = engine.load_library(); vp = C.c_void_p
         self.sinks = list(sinks)
         arr = (vp * len(self.sinks))(*[s._h for s in self.sinks])
         self._h = vp(); self._keep = {}
