@@ -140,6 +140,7 @@ typedef struct tf_batch {
 #define TF_ROWERR_CSV_BAD_FLOAT    22
 #define TF_ROWERR_CSV_UNSUPPORTED  23 /* valid for Go's parsers, but a syntax the device does not implement   */
 #define TF_ROWERR_CSV_DQ_DISABLED  24 /* reader.go:305-311 errDoubleQuotesDisabled                           */
+#define TF_ROWERR_CSV_QUOTING_DISABLED 25 /* reader.go:185-187 errQuotingDisabled: a '"' on a line read with "quote":"" */
 
 /* generic JSON parser (tfgpu_parse_json) */
 #define TF_ROWERR_JSON_PARSE        32 /* fastjson rejects the line -> unparsed row (generic_parser.go:548-553)            */
@@ -317,11 +318,15 @@ int tfgpu_measure(tfgpu_engine* e, const tf_batch* in, uint64_t* per_row, uint64
 
 /* parsers.Parser for CSV (pkg/parsers/abstract.go:35-38 shape; algorithm of the S3 CSV reader:
  * pkg/csv/reader.go:89-324 + pkg/providers/s3/reader/registry/csv/reader_csv.go:186-452 + strictify.go:18-181).
- * One chunk of raw bytes (host or device, < 4 GiB) is split into lines and typed columns ON THE DEVICE and fed straight
+ * One chunk of raw bytes (host, or device memory at any alignment, < 4 GiB) is split into lines and typed columns ON THE DEVICE and fed straight
  * into the plan's transformer chain; wire_fmt 0 returns the Transformed rows columnar (tfgpu_result_batch), otherwise the
  * sink wire bytes. The schema's `path` of each column is the field index (reader_csv.go:286); opts_json:
  * {"delimiter":",","quote":"\"","escape":"\\","double_quote":true,"null_values":[..],"strings_can_be_null":false,
  *  "quoted_strings_can_be_null":false,"true_values":[..],"false_values":[..],"include_missing_columns":false,"skip_lines":0}.
+ * Inside an element, the quote character written twice stands for one '"' (the S3 reader's DoubleQuoteStr = quote + quote,
+ * swapToSingleQuotes reader.go:309-324), whatever the quote character is; with "double_quote":false such a pair is
+ * TF_ROWERR_CSV_DQ_DISABLED. With "quote":"" a data line that contains '"' is TF_ROWERR_CSV_QUOTING_DISABLED, which outranks
+ * every other error of the line; lines dropped by skip_lines are not checked (in the reference such a line fails the whole read).
  * Row-level failures come back as row errors with TF_ROWERR_CSV_* codes (row = data line index); an unterminated last
  * line is left unconsumed (tfgpu_result_consumed) exactly as the reference drops it (reader.go:162-165). */
 int tfgpu_parse_csv(tfgpu_engine* e, int plan_id, const char* opts_json, const uint8_t* bytes, uint64_t len, int mem,

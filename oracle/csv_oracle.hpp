@@ -24,7 +24,7 @@
 namespace orc {
 
 enum CsvErr { CSV_OK = 0, CSV_MISSING_CELL = 16, CSV_SINGLE_QUOTE = 17, CSV_BAD_INT = 18, CSV_RANGE = 19, CSV_BAD_BOOL = 20,
-              CSV_BAD_TIME = 21, CSV_BAD_FLOAT = 22, CSV_UNSUPPORTED = 23, CSV_DOUBLE_QUOTE_DISABLED = 24 };
+              CSV_BAD_TIME = 21, CSV_BAD_FLOAT = 22, CSV_UNSUPPORTED = 23, CSV_DOUBLE_QUOTE_DISABLED = 24, CSV_QUOTING_DISABLED = 25 };
 
 struct CsvOpts {
     uint8_t delimiter = ',', quote = '"', escape = '\\';
@@ -243,9 +243,10 @@ inline int csv_split(const CsvOpts& o, const uint8_t* line, size_t n, std::vecto
             if (m == 1 && p[0] == o.quote) return CSV_SINGLE_QUOTE;                 // unquote :287-301
             if (m >= 2 && p[0] == o.quote && p[m - 1] == o.quote) { p++; m -= 2; }
             el.assign((const char*)p, m);
-            bool has = el.find("\"\"") != std::string::npos;                        // swapToSingleQuotes :305-318 (DoubleQuoteStr is `""`)
+            const std::string pair(2, (char)o.quote);                                  // DoubleQuoteStr = quote + quote (s3 csv_config.go:141)
+            bool has = el.find(pair) != std::string::npos;                             // swapToSingleQuotes :309-324: ReplaceAll(el, pair, `"`)
             if (has && !o.double_quote) return CSV_DOUBLE_QUOTE_DISABLED;
-            if (has) { had_dq.back() = 1; std::string r; for (size_t i = 0; i < el.size(); i++) { if (el[i] == '"' && i + 1 < el.size() && el[i + 1] == '"') { r += '"'; i++; } else r += el[i]; } el.swap(r); }
+            if (has) { had_dq.back() = 1; std::string r; for (size_t i = 0; i < el.size(); i++) { if (el.compare(i, 2, pair) == 0) { r += '"'; i++; } else r += el[i]; } el.swap(r); }
         } else el.assign((const char*)p, m);
         return 0;
     };
@@ -276,7 +277,8 @@ inline CsvResult csv_parse(const uint8_t* buf, size_t len, const std::vector<Csv
         const uint64_t ln = line_no++;
         if (ln < skip_lines) continue;
         int err = 0;
-        if (n == 1) { cells.clear(); had_dq.clear(); }                     // "\n": ReadLine returns no entries (:141-145)
+        if (!o.quote && std::memchr(line, '"', n)) err = CSV_QUOTING_DISABLED;     // readAndDecodeLine :185-187, before the split
+        else if (n == 1) { cells.clear(); had_dq.clear(); }                   // "\n": ReadLine returns no entries (:141-145)
         else err = csv_split(o, line, n, cells, had_dq);
         std::vector<std::array<uint8_t, 8>> vals(schema.size()); std::vector<uint32_t> ns(schema.size(), 0); std::vector<std::string> sv(schema.size()); std::vector<int> tag(schema.size(), 1);
         // constructCI (reader_csv.go:266-343) visits every column first: a missing cell outranks conversion errors,

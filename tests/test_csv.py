@@ -36,6 +36,14 @@ def test_reader_reference_cases(po):
     # the reference takes line[lastDelimPosition+1:] for the last element, i.e. line[1:] when there is no delimiter
     b, e, _, _ = po.csv_parse(b"abc\n", S(1))
     assert cells(b) == [[b"bc"]]
+    # DoubleQuoteStr is the quote character twice (s3 csv_config.go:141); swapToSingleQuotes turns it into `"` whatever the quote is
+    b, e, _, _ = po.csv_parse(b"a,'it''s'\nb,x\"\"y\n", S(2), {"quote": "'"})
+    assert cells(b) == [[b"a", b'it"s'], [b"b", b'x""y']] and not e
+    b, e, _, _ = po.csv_parse(b"a,'it''s'\nb,x\"\"y\n", S(2), {"quote": "'", "double_quote": False})
+    assert cells(b) == [[b"b", b'x""y']] and e == [(0, 24, 0)]
+    # no quote character: a line holding `"` fails in readAndDecodeLine (reader.go:185-187), before any other check of the line
+    b, e, _, _ = po.csv_parse(b'a,x"y\n"\nb\nc,d\n', S(2), {"quote": ""})
+    assert cells(b) == [[b"c", b"d"]] and e == [(0, 25, 0), (1, 25, 0), (2, 16, 0)]
 
 
 def test_typed_cells_and_errors(po):
@@ -168,6 +176,9 @@ def test_device_csv_cases_and_errors(eng, po):
         (b'a, b, "the main ""test"" is this", d\n', S(4), None), (b'a, b, "the main ""test"" is this", d\n', S(4), {"double_quote": False}),
         (b"a,b\nc,d", S(2), None), (b'a,"\nx,y\n', S(2), None), (b"abc\n\n\r\nq\n", S(1), {"include_missing_columns": True}),
         (b"h1;h2\n1;\xc2\xa0 spaced \xe3\x80\x80\n", S(2), {"delimiter": ";", "skip_lines": 1}), (b"", S(2), None), (b"no newline", S(1), None),
+        (b"a,'it''s'\nb,x\"\"y\nc,'''',''\nd,'x''''\n", S(2), {"quote": "'"}), (b"a,'it''s'\nb,x\"\"y\n", S(2), {"quote": "'", "double_quote": False}),
+        (b"k,'it''s',x\"\"y," + b",".join(b"%d" % f for f in range(260)) + b"\n", S(3), {"quote": "'"}),      # 263 fields: the sequential path
+        (b'a,x"y\n"\nb\nc,d\n"h",1\nq,r\n', S(2), {"quote": "", "skip_lines": 1}),
     ]
     sch = [{"name": "i", "type": "int32", "path": "0"}, {"name": "t", "type": "timestamp", "path": "1"}, {"name": "d", "type": "date", "path": "2"},
            {"name": "f", "type": "double", "path": "3"}, {"name": "b", "type": "boolean", "path": "4"}, {"name": "u", "type": "uint8", "path": "5"},

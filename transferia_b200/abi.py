@@ -104,7 +104,7 @@ TF_WIRE_SER_JSON, TF_WIRE_SER_CSV = 4, 5
 TF_WIRE_F_CLOSING_NEWLINE, TF_WIRE_F_ANY_AS_STRING = 0x100, 0x200
 TF_WIRE_F_GZIP, TF_WIRE_F_ZLIB = 0x400, 0x800     # the row text as one gzip member / zlib stream (include/tfgpu.h)
 TF_WIRE_DEBEZIUM = 6
-TF_ROWERR_CSV_BAD_FLOAT, TF_ROWERR_CSV_UNSUPPORTED = 22, 23
+TF_ROWERR_CSV_BAD_FLOAT, TF_ROWERR_CSV_UNSUPPORTED, TF_ROWERR_CSV_DQ_DISABLED, TF_ROWERR_CSV_QUOTING_DISABLED = 22, 23, 24, 25
 TF_ROWERR_N2F_HOST = 52
 TF_ROWERR_DBZ_EMIT_HOST = 53
 TF_ROWERR_SINK_KIND_HOST = 54

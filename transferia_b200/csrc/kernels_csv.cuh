@@ -6,8 +6,8 @@
 // In single-line mode the quote state resets at every '\n' (reader.go:137-155), so lines are independent:
 //   k_csv_count_nl / k_csv_line_index   newline index (count per 8 KiB block, scan, positions)
 //   k_csv_pass1   one thread per line: the reference's split state machine (escape-inside-quotes, quote toggle,
-//                 delimiter outside quotes, the `line[lastDelim+1:]` last-element rule), TrimSpace, unquote, `""`
-//                 collapse; fixed-width cells are converted and stored column-major (coalesced across lines),
+//                 delimiter outside quotes, the `line[lastDelim+1:]` last-element rule), TrimSpace, unquote, the collapse of
+//                 a doubled quote character (DoubleQuoteStr = quote + quote) into `"`; fixed-width cells are converted and stored column-major (coalesced across lines),
 //                 text cells leave (start, length) spans
 //   k_csv_offsets per text column: exclusive scan of lengths -> uint32 offsets
 //   k_csv_pass2   copy text cells into the column heaps
@@ -19,7 +19,8 @@
 namespace tfk {
 
 enum CsvErr : int { CSV_MISSING_CELL = 16, CSV_SINGLE_QUOTE = 17, CSV_BAD_INT = 18, CSV_RANGE = 19, CSV_BAD_BOOL = 20,
-                    CSV_BAD_TIME = 21, CSV_BAD_FLOAT = 22, CSV_UNSUPPORTED = 23, CSV_DOUBLE_QUOTE_DISABLED = 24 };
+                    CSV_BAD_TIME = 21, CSV_BAD_FLOAT = 22, CSV_UNSUPPORTED = 23, CSV_DOUBLE_QUOTE_DISABLED = 24,
+                    CSV_QUOTING_DISABLED = 25 };
 
 #define CSV_NL_BLOCK 8192
 
@@ -46,7 +47,8 @@ struct CsvArgs {
     const CsvColDev* cols; int ncols;
     const int16_t* field_col; int nfields;       // first schema column that reads field f, -1 none
     const int16_t* next_same;                    // next schema column with the same path, -1 none
-    uint32_t* span_start; uint32_t* span_len;    // [nslots][nrows]; len bit31 = contains `""` (collapse on copy)
+    uint32_t* span_start; uint32_t* span_len;    // [nslots][nrows]; len bit31 = contains a doubled quote (collapse on copy)
+    uint32_t* span_raw;                          // [nslots][nrows]; the uncollapsed length of a bit31 span (set only for those)
     uint8_t* err;                                // [nrows] CSV_* code
 };
 
@@ -248,7 +250,7 @@ __device__ __forceinline__ void csv_store_fixed(const CsvColDev& c, uint64_t row
 // getCorrespondingValue + strictifyValue for one cell [p, p+n) (already sanitised); text cells return their span
 static __device__ int csv_cell(const CsvArgs& a, const CsvColDev& c, uint64_t row, uint64_t nrows, const uint8_t* p, uint32_t n, bool has_dq) {
     const CsvCfg& o = a.cfg;
-    if (has_dq && c.w) return CSV_UNSUPPORTED;       // a `""` inside a numeric cell: the collapsed text would have to be materialised first
+    if (has_dq && c.w) return CSV_UNSUPPORTED;       // a doubled quote inside a numeric cell: the collapsed text would have to be materialised first
     switch (c.tf) {
     case TF_BOOLEAN: {
         bool b;
@@ -291,8 +293,9 @@ static __device__ int csv_cell(const CsvArgs& a, const CsvColDev& c, uint64_t ro
         uint32_t* ss = a.span_start + (size_t)c.slot * nrows; uint32_t* sl = a.span_len + (size_t)c.slot * nrows;
         if (null) { if (c.tf == TF_ANY) { ss[row] = 0xffffffffu; sl[row] = 2; c.aux8[row] = 0; } else { ss[row] = 0; sl[row] = 0; } return 0; }
         uint32_t fl = n;
-        if (has_dq) { uint32_t k = 0; fl = 0; while (k < n) { if (p[k] == '"' && k + 1 < n && p[k + 1] == '"') k += 2; else k++; fl++; } }
+        if (has_dq) { const uint8_t q = o.quote; uint32_t k = 0; fl = 0; while (k < n) { if (p[k] == q && k + 1 < n && p[k + 1] == q) k += 2; else k++; fl++; } }
         ss[row] = (uint32_t)(p - a.text); sl[row] = fl | (has_dq ? 0x80000000u : 0u);
+        if (has_dq) a.span_raw[(size_t)c.slot * nrows + row] = n;
         if (c.tf == TF_ANY) c.aux8[row] = 1;
         return 0;
     }
@@ -334,7 +337,7 @@ static __device__ void csv_row_sequential(const CsvArgs& a, uint64_t row, uint64
         if (o.quote) {
             if (m == 1 && p[0] == o.quote) { err = CSV_SINGLE_QUOTE; return; }
             if (m >= 2 && p[0] == o.quote && p[m - 1] == o.quote) { p++; m -= 2; }
-            for (uint32_t k = 0; k + 1 < m; k++) if (p[k] == '"' && p[k + 1] == '"') { has_dq = true; break; }
+            for (uint32_t k = 0; k + 1 < m; k++) if (p[k] == o.quote && p[k + 1] == o.quote) { has_dq = true; break; }
             if (has_dq && !o.double_quote) { err = CSV_DOUBLE_QUOTE_DISABLED; return; }
         }
         if (f < a.nfields) for (int c = a.field_col[f]; c >= 0; c = a.next_same[c]) {
@@ -342,7 +345,8 @@ static __device__ void csv_row_sequential(const CsvArgs& a, uint64_t row, uint64
             if (rc && c < conv_col) { conv_col = c; conv_err = rc; }
         }
     };
-    if (n > 1) {
+    if (!o.quote) for (uint32_t i = 0; i < n; i++) if (line[i] == '"') { err = CSV_QUOTING_DISABLED; break; }      // readAndDecodeLine (reader.go:185-187), before the split
+    if (n > 1 && !err) {
         uint8_t prev = 0; bool inq = false; uint32_t prev_delim = 0, last_delim = 0;
         for (uint32_t i = 0; i < n && !err; i++) {
             const uint8_t c = line[i];
@@ -385,7 +389,7 @@ static __device__ void csv_rows_by_warp(const CsvArgs& a, uint64_t row0, uint64_
         const uint32_t ls = ln ? a.line_end[ln - 1] : 0, le = a.line_end[ln];
         const uint8_t* line = a.text + ls; const uint32_t n = le - ls;
         // ---- tokenise
-        uint32_t nd = 0;
+        uint32_t nd = 0, dq = 0;         // dq: a '"' on a line read without a quote character
         if (lane <= CSV_MAXF / 32) s_fq[warp][lane] = 0;
         __syncwarp();
         if (n > 1) {
@@ -393,6 +397,7 @@ static __device__ void csv_rows_by_warp(const CsvArgs& a, uint64_t row0, uint64_
             for (uint32_t base = 0; base < n; base += 32) {
                 const uint32_t i = base + lane; const bool in = i < n;
                 const uint32_t c = in ? line[i] : 0u;
+                if (!o.quote) dq |= __ballot_sync(0xffffffffu, c == '"');
                 const uint32_t up = __shfl_up_sync(0xffffffffu, c, 1); const uint32_t prev = lane ? up : prevc;
                 const bool isq = in && o.quote && c == o.quote;
                 const uint32_t qm = __ballot_sync(0xffffffffu, isq);
@@ -413,8 +418,8 @@ static __device__ void csv_rows_by_warp(const CsvArgs& a, uint64_t row0, uint64_
             }
         }
         __syncwarp();
-        if (nd > CSV_MAXF) { if (lane == 0) csv_row_sequential(a, row, nrows); __syncwarp(); continue; }      // more delimiters than the table holds
-        const uint32_t nf = n > 1 ? nd + 1 : 0;
+        if (nd > CSV_MAXF && !dq) { if (lane == 0) csv_row_sequential(a, row, nrows); __syncwarp(); continue; }      // more delimiters than the table holds
+        const uint32_t nf = n > 1 && !dq ? nd + 1 : 0;
         // ---- elements, 32 at a time
         uint32_t err_key = 0xffffffffu, conv_key = 0xffffffffu;      // (field << 8) | code of the first split-level error; (column << 8) | code of the first conversion error
         for (uint32_t f = lane; f < nf; f += 32) {
@@ -427,7 +432,7 @@ static __device__ void csv_rows_by_warp(const CsvArgs& a, uint64_t row0, uint64_
                 if (m == 1 && p[0] == o.quote) e = CSV_SINGLE_QUOTE;
                 else {
                     if (m >= 2 && p[0] == o.quote && p[m - 1] == o.quote) { p++; m -= 2; }
-                    for (uint32_t k = 0; k + 1 < m; k++) if (p[k] == '"' && p[k + 1] == '"') { has_dq = true; break; }
+                    for (uint32_t k = 0; k + 1 < m; k++) if (p[k] == o.quote && p[k + 1] == o.quote) { has_dq = true; break; }
                     if (has_dq && !o.double_quote) e = CSV_DOUBLE_QUOTE_DISABLED;
                 }
             }
@@ -438,7 +443,7 @@ static __device__ void csv_rows_by_warp(const CsvArgs& a, uint64_t row0, uint64_
             }
         }
         err_key = __reduce_min_sync(0xffffffffu, err_key); conv_key = __reduce_min_sync(0xffffffffu, conv_key);
-        int err = err_key == 0xffffffffu ? 0 : (int)(err_key & 0xff);
+        int err = dq ? CSV_QUOTING_DISABLED : err_key == 0xffffffffu ? 0 : (int)(err_key & 0xff);      // (raised before the split: outranks the rest)
         // columns whose field is missing, or that take the default value (reader_csv.go:291-313). constructCI runs over
         // every column before Strictify does, so a missing cell outranks any conversion error.
         bool missing = false;
@@ -488,11 +493,12 @@ __global__ void __launch_bounds__(32 * CSV_WARPS, 4) k_csv_pass1(CsvArgs a) {
         {
             const uint32_t mis = (uint32_t)((uintptr_t)(a.text + g0) & 15);       // 16-byte chunks of the text, aligned in global memory
             const uint8_t* gb = a.text + g0 - mis; const uint32_t nchunk = (mis + (g1 - g0) + 15) >> 4;
+            const int64_t gs = (int64_t)g0 - (int64_t)mis;      // text offset of s_tile[0]: negative in the first tile of a text that starts misaligned
             for (uint32_t c = threadIdx.x; c < nchunk; c += blockDim.x) {
-                const uint32_t off = c * 16;
-                // the tile is kept at the same misalignment: s_tile[mis + k] = text[g0 + k]
-                if ((uint64_t)(g0 - mis) + off + 16 <= a.len) *(int4*)(s_tile + off) = __ldg((const int4*)(gb + off));
-                else for (uint32_t b = 0; b < 16; b++) s_tile[off + b] = ((uint64_t)(g0 - mis) + off + b < a.len) ? gb[off + b] : 0;      // the end of the text
+                const uint32_t off = c * 16; const int64_t t = gs + off;
+                // the tile is kept at the same misalignment: s_tile[mis + k] = text[g0 + k]; bytes outside [0, len) of the text are zeros
+                if (t >= 0 && t + 16 <= (int64_t)a.len) *(int4*)(s_tile + off) = __ldg((const int4*)(gb + off));
+                else for (uint32_t b = 0; b < 16; b++) s_tile[off + b] = (t + b >= 0 && t + b < (int64_t)a.len) ? gb[off + b] : 0;
             }
             if (threadIdx.x <= nr) s_ls[threadIdx.x] = (threadIdx.x ? a.line_end[ln0 + threadIdx.x - 1] : g0) - g0 + mis;
             if (threadIdx.x < CSV_TILE_ROWS) { s_errk[threadIdx.x] = 0xffffffffu; s_convk[threadIdx.x] = 0xffffffffu; s_miss[threadIdx.x] = 0; s_nd[threadIdx.x] = 0; }
@@ -502,12 +508,13 @@ __global__ void __launch_bounds__(32 * CSV_WARPS, 4) k_csv_pass1(CsvArgs a) {
         // ---- tokenise: warp w takes lines w, w + 8, ...
         for (uint32_t r = warp; r < nr; r += CSV_WARPS) {
             const uint8_t* line = s_tile + s_ls[r]; const uint32_t n = s_ls[r + 1] - s_ls[r];
-            uint32_t nd = 0;
+            uint32_t nd = 0, dq = 0;        // dq: a '"' on a line read without a quote character
             if (n > 1) {
                 uint32_t inq_carry = 0, prevc = 0;
                 for (uint32_t base = 0; base < n; base += 32) {
                     const uint32_t i = base + lane; const bool in = i < n;
                     const uint32_t c = in ? line[i] : 0u;
+                    if (!o.quote) dq |= __ballot_sync(0xffffffffu, c == '"');
                     const uint32_t up = __shfl_up_sync(0xffffffffu, c, 1); const uint32_t prev = lane ? up : prevc;
                     const bool isq = in && o.quote && c == o.quote;
                     const uint32_t qm = __ballot_sync(0xffffffffu, isq);
@@ -527,13 +534,13 @@ __global__ void __launch_bounds__(32 * CSV_WARPS, 4) k_csv_pass1(CsvArgs a) {
                     prevc = __shfl_sync(0xffffffffu, c, 31);
                 }
             }
-            if (lane == 0) s_nd[r] = nd | (n > 1 ? 0x80000000u : 0u);
+            if (lane == 0) s_nd[r] = nd | (n > 1 ? 0x80000000u : 0u) | (dq ? 0x40000000u : 0u);      // (nd < 2^30: a tile holds 28672 bytes)
         }
         __syncthreads();
         // ---- elements: lane = line, the warps stride over the element index
         {
             const uint32_t r = lane; const bool live = r < nr;
-            const uint32_t ndw = live ? s_nd[r] : 0; const uint32_t nd = ndw & 0x7fffffffu; const uint32_t nf = (ndw >> 31) ? nd + 1 : 0;
+            const uint32_t ndw = live ? s_nd[r] : 0; const uint32_t nd = ndw & 0x3fffffffu; const uint32_t nf = (ndw >> 31) && !(ndw & 0x40000000u) ? nd + 1 : 0;
             const uint32_t n = live ? s_ls[r + 1] - s_ls[r] : 0;
             const uint8_t* line = s_tile + (live ? s_ls[r] : 0);
             const uint64_t row = row0 + r;
@@ -555,7 +562,7 @@ __global__ void __launch_bounds__(32 * CSV_WARPS, 4) k_csv_pass1(CsvArgs a) {
                     if (m == 1 && p[0] == o.quote) e = CSV_SINGLE_QUOTE;
                     else {
                         if (m >= 2 && p[0] == o.quote && p[m - 1] == o.quote) { p++; m -= 2; }
-                        for (uint32_t k = 0; k + 1 < m; k++) if (p[k] == '"' && p[k + 1] == '"') { has_dq = true; break; }
+                        for (uint32_t k = 0; k + 1 < m; k++) if (p[k] == o.quote && p[k + 1] == o.quote) { has_dq = true; break; }
                         if (has_dq && !o.double_quote) e = CSV_DOUBLE_QUOTE_DISABLED;
                     }
                 }
@@ -581,7 +588,8 @@ __global__ void __launch_bounds__(32 * CSV_WARPS, 4) k_csv_pass1(CsvArgs a) {
             int err = 0;
             if (live) {
                 const uint32_t ndw = s_nd[r];
-                if ((ndw & 0x7fffffffu) > CSV_TF) err = -1;                // more delimiters than the table holds: redo this line sequentially
+                if (ndw & 0x40000000u) err = CSV_QUOTING_DISABLED;         // raised before the split: outranks every other error of the line
+                else if ((ndw & 0x3fffffffu) > CSV_TF) err = -1;           // more delimiters than the table holds: redo this line sequentially
                 else if (s_errk[r] != 0xffffffffu) err = (int)(s_errk[r] & 0xff);
                 else if (s_miss[r]) err = CSV_MISSING_CELL;
                 else if (s_convk[r] != 0xffffffffu) err = (int)(s_convk[r] & 0xff);
@@ -662,7 +670,8 @@ __global__ void __launch_bounds__(1024) k_offsets_write(const uint32_t* span_len
 }
 #endif  // TF_KERNELS_CSV
 
-struct CsvCopyArgs { const uint8_t* text; const uint32_t* span_start; const uint32_t* span_len; const uint32_t* offsets; uint8_t* heap; const uint64_t* col_base; uint64_t nrows; };
+struct CsvCopyArgs { const uint8_t* text; const uint32_t* span_start; const uint32_t* span_len; const uint32_t* span_raw; const uint32_t* offsets; uint8_t* heap;
+                     const uint64_t* col_base; uint64_t nrows; uint8_t quote; };      // a doubled quote character in a flagged span is copied as one '"' (swapToSingleQuotes)
 
 #ifdef TF_KERNELS_CSV
 __global__ void __launch_bounds__(256) k_csv_pass2(CsvCopyArgs a) {
@@ -675,7 +684,10 @@ __global__ void __launch_bounds__(256) k_csv_pass2(CsvCopyArgs a) {
     uint8_t* o = a.heap + a.col_base[slot] + a.offsets[(size_t)slot * (a.nrows + 1) + row];
     if (st == 0xffffffffu) { o[0] = '{'; o[1] = '}'; return; }
     const uint8_t* s = a.text + st;
-    if (lf & 0x80000000u) { uint32_t k = 0; for (uint32_t w = 0; w < L; w++) { o[w] = s[k]; k += (s[k] == '"' && s[k + 1] == '"') ? 2 : 1; } }
+    if (lf & 0x80000000u) {      // (a pair may not take the byte after the span: that can be the quote unquote stripped)
+        const uint8_t q = a.quote; const uint32_t R = a.span_raw[(size_t)slot * a.nrows + row]; uint32_t k = 0;
+        for (uint32_t w = 0; w < L; w++) { const bool pair = k + 1 < R && s[k] == q && s[k + 1] == q; o[w] = pair ? '"' : s[k]; k += pair ? 2 : 1; }
+    }
     else for (uint32_t k = 0; k < L; k++) o[k] = s[k];
 }
 #endif  // TF_KERNELS_CSV

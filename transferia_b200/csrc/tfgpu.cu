@@ -1360,7 +1360,7 @@ int tfgpu_parse_csv(tfgpu_engine* e, int plan_id, const char* opts_json, const u
         for (int c = (int)nc - 1; c >= 0; c--) if (hc[c].path >= 0) { next_same[c] = field_col[hc[c].path]; field_col[hc[c].path] = (int16_t)c; }
         Layout L;
         const size_t o_line = L.take((nlines + 1) * 4), o_err = L.take(nrows), o_cols = L.take(nc * sizeof(CsvColDev)), o_fc = L.take(field_col.size() * 2), o_ns = L.take(nc * 2),
-                     o_blob = L.take(ho.blob.size()), o_ss = L.take((size_t)nslots * nrows * 4), o_sl = L.take((size_t)nslots * nrows * 4),
+                     o_blob = L.take(ho.blob.size()), o_ss = L.take((size_t)nslots * nrows * 4), o_sl = L.take((size_t)nslots * nrows * 4), o_sr = L.take((size_t)nslots * nrows * 4),
                      o_off = L.take((size_t)nslots * (nrows + 1) * 4), o_tot = L.take((size_t)nslots * 8 + 8), o_base = L.take((size_t)nslots * 8 + 8);
         std::vector<size_t> o_val(nc), o_aux(nc);
         for (size_t c = 0; c < nc; c++) {
@@ -1384,14 +1384,14 @@ int tfgpu_parse_csv(tfgpu_engine* e, int plan_id, const char* opts_json, const u
         if (nlines) { e->prof_begin("k_csv_line_index", s); launch_k_csv_line_index(nblk, 256, 0, s, d_text, len, blk_off, (uint32_t*)(B + o_line), nullptr); e->prof_end(s); }
         if (nrows) {
             CsvArgs ca{d_text, len, (const uint32_t*)(B + o_line), nlines, skip, ho.cfg, B + o_blob, (const CsvColDev*)(B + o_cols), (int)nc,
-                       (const int16_t*)(B + o_fc), nfields, (const int16_t*)(B + o_ns), (uint32_t*)(B + o_ss), (uint32_t*)(B + o_sl), B + o_err};
+                       (const int16_t*)(B + o_fc), nfields, (const int16_t*)(B + o_ns), (uint32_t*)(B + o_ss), (uint32_t*)(B + o_sl), (uint32_t*)(B + o_sr), B + o_err};
             e->prof_begin("k_csv_pass1", s); launch_k_csv_pass1((uint32_t)std::min<uint64_t>((nrows + CSV_TILE_ROWS - 1) / CSV_TILE_ROWS, (uint64_t)e->sm_count * 16), 32 * CSV_WARPS, 0, s, ca); e->prof_end(s);
             if (nslots) {
                 // text heaps (the staged batch lives in csv_stage, in_arena is free)
                 h = size_heaps(e, (const uint32_t*)(B + o_sl), nrows, (uint32_t)nslots, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), (uint64_t*)(B + o_base),
                                e->in_arena, "csv chunk: a text column exceeds 4 GiB");
                 heap = e->in_arena.p;
-                CsvCopyArgs cp{d_text, (const uint32_t*)(B + o_ss), (const uint32_t*)(B + o_sl), (const uint32_t*)(B + o_off), e->in_arena.p, (const uint64_t*)(B + o_base), nrows};
+                CsvCopyArgs cp{d_text, (const uint32_t*)(B + o_ss), (const uint32_t*)(B + o_sl), (const uint32_t*)(B + o_sr), (const uint32_t*)(B + o_off), e->in_arena.p, (const uint64_t*)(B + o_base), nrows, ho.cfg.quote};
                 e->prof_begin("k_csv_pass2", s); launch_k_csv_pass2(dim3((uint32_t)((nrows + 255) / 256), nslots), 256, 0, s, cp); e->prof_end(s);
             }
         }

@@ -296,20 +296,26 @@ class Engine:
             self._L.tfgpu_result_release(res)
 
     @staticmethod
-    def _host_bytes(data):
-        """(pointer, length, keepalive) of a bytes object or a (pinned) torch uint8 tensor, without copying."""
+    def _input_bytes(data):
+        """(pointer, length, TF_MEM_*, keepalive) of a bytes object or a contiguous torch uint8 tensor, without copying. A CUDA tensor
+        (any offset into its storage) is read in place on the device after the work queued on its stream has finished; a (pinned)
+        host tensor stays host memory."""
         if hasattr(data, "data_ptr"):
-            return C.c_void_p(data.data_ptr()), int(data.numel()), data
+            if data.is_cuda:
+                import torch
+                torch.cuda.current_stream(data.device).synchronize()     # the engine reads it on its own stream
+                return C.c_void_p(data.data_ptr()), int(data.numel()), abi.TF_MEM_DEVICE, data
+            return C.c_void_p(data.data_ptr()), int(data.numel()), abi.TF_MEM_HOST, data
         buf = C.c_char_p(data if data else b"\0")              # the bytes object's own storage
-        return C.cast(buf, C.c_void_p), len(data), buf
+        return C.cast(buf, C.c_void_p), len(data), abi.TF_MEM_HOST, buf
 
     def parse_csv(self, plan_id: int, data, opts: Optional[dict] = None, wire_fmt: int = 0, copy_bytes: bool = True):
-        """CSV bytes (a bytes object or a pinned torch uint8 tensor, used in place) -> typed columns -> the plan's transformer chain, all on
+        """CSV bytes (a bytes object, a pinned or a CUDA torch uint8 tensor, used in place) -> typed columns -> the plan's transformer chain, all on
         the device. wire_fmt 0: (Batch, row errors, consumed bytes); otherwise (PushResult, consumed bytes); copy_bytes=False leaves the
         wire bytes in the engine's pinned landing buffer and only reports their length."""
-        ptr, total, keep = self._host_bytes(data)
+        ptr, total, mem, keep = self._input_bytes(data)
         res = C.c_void_p()
-        self._check(self._L.tfgpu_parse_csv(self._h, plan_id, json.dumps(opts or {}).encode(), ptr, total, abi.TF_MEM_HOST, wire_fmt, C.byref(res)))
+        self._check(self._L.tfgpu_parse_csv(self._h, plan_id, json.dumps(opts or {}).encode(), ptr, total, mem, wire_fmt, C.byref(res)))
         try:
             consumed = int(self._L.tfgpu_result_consumed(res))
             if wire_fmt == 0:
@@ -326,9 +332,9 @@ class Engine:
         per MESSAGE, selection per output row); otherwise (PushResult, meta)."""
         ends = np.asarray(msg_ends, dtype=np.uint64)
         opts = {"schema_text": schema_text, "schema_registry": schema_registry, "schema_id": schema_id, "check_table": check_table}
-        ptr, total, keep = self._host_bytes(data)
+        ptr, total, mem, keep = self._input_bytes(data)
         res = C.c_void_p()
-        self._check(self._L.tfgpu_parse_debezium(self._h, plan_id, json.dumps(opts).encode(), ptr, total, abi.TF_MEM_HOST, ends.ctypes.data, len(ends), wire_fmt, C.byref(res)))
+        self._check(self._L.tfgpu_parse_debezium(self._h, plan_id, json.dumps(opts).encode(), ptr, total, mem, ends.ctypes.data, len(ends), wire_fmt, C.byref(res)))
         try:
             L = self._L
             nin, nout = int(L.tfgpu_result_rows_in(res)), int(L.tfgpu_result_rows_out(res))
@@ -383,13 +389,13 @@ class Engine:
         msgs: [(end, offset, write_sec, write_nsec)] (default: one message = all of `data`).
         wire_fmt 0: (Batch, row errors, non-empty lines); otherwise PushResult (copy_bytes=False leaves the wire bytes in the
         engine's pinned landing buffer and only reports their length)."""
-        ptr, total, keep = self._host_bytes(data)
+        ptr, total, mem, keep = self._input_bytes(data)
         msgs = msgs if msgs is not None else [(total, 0, 0, 0)]
         ms = (abi.TfMsg * max(1, len(msgs)))()
         for k, (end, off, ws, wn) in enumerate(msgs):
             ms[k].end, ms[k].offset, ms[k].write_sec, ms[k].write_nsec = end, off, ws, wn
         res = C.c_void_p()
-        self._check(self._L.tfgpu_parse_json(self._h, plan_id, json.dumps(opts or {}).encode(), ptr, total, abi.TF_MEM_HOST, ms, len(msgs), wire_fmt, C.byref(res)))
+        self._check(self._L.tfgpu_parse_json(self._h, plan_id, json.dumps(opts or {}).encode(), ptr, total, mem, ms, len(msgs), wire_fmt, C.byref(res)))
         try:
             if wire_fmt == 0:
                 b, errs = self._result_batch(res)
