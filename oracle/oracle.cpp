@@ -211,7 +211,7 @@ int match_value(const orc_val& v1, const orc_term& t, bool& matched) {
             return ordered<int64_t>(int1, t.i, op, matched) ? 0 : TF_ROWERR_FILTER_TYPEPAIR;
         }
         if (is_float1) {
-            if (is_set) { if (std::trunc(float1) == float1) return set_res(in_ilist((int64_t)float1)); matched = false; return 0; }
+            if (is_set) { if (std::trunc(float1) == float1) return set_res(in_ilist(gocast::go_f2i64(float1))); matched = false; return 0; }   // int64(float1): amd64 CVTTSD2SQ
             return ordered<double>(float1, (double)t.i, op, matched) ? 0 : TF_ROWERR_FILTER_TYPEPAIR;
         }
         break;

@@ -14,6 +14,7 @@ Python front of the CPU oracle:
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 import re
 import subprocess
@@ -328,7 +329,11 @@ def parse_filter(src: str) -> List[Term]:
         if is_kw((kind, text), "TRUE", "FALSE"):
             p += 1; return LV_BOOL, text.upper() == "TRUE"
         if kind == "Float":
-            p += 1; return LV_FLOAT, float(text)
+            p += 1
+            v = float(text)
+            if math.isinf(v):                                   # strconv.ParseFloat: ErrRange beyond the float64 range
+                raise FilterSyntaxError("value out of range")
+            return LV_FLOAT, v
         if kind == "Int":
             p += 1
             v = int(text)

@@ -153,6 +153,7 @@ static __device__ int eval_term(const RowVal& v, const DTerm& t, const uint8_t* 
     const int op = t.op; const bool is_set = (op == 6 || op == 7);
     const int base = t.vtype & 15; const bool is_list = (t.vtype & 16) != 0;
     if (v.cls == 8) return TF_ROWERR_FILTER_OVERFLOW;                       // filter_rows.go:193-197
+    if (op >= 8 && base != 4) return TF_ROWERR_FILTER_TYPEPAIR;             // ~ / !~ on a non-string literal: matchOrderedValue has no such operation (:367-383)
     const bool is_int1 = v.cls == 1;
     const bool is_float1 = v.cls == 2 || v.cls == 3 || v.cls == 0;          // cast.ToFloat64E: floats, bool, nil (-> 0)
     const double float1 = v.cls == 2 ? v.f : (v.cls == 3 ? v.f : 0.0);
@@ -165,8 +166,8 @@ static __device__ int eval_term(const RowVal& v, const DTerm& t, const uint8_t* 
             matched = ordered<int64_t>(v.i, t.i, op); return 0;
         }
         if (is_float1) {
-            if (is_set) {
-                if (trunc(float1) == float1) { int64_t x = (int64_t)float1; bool c = false; for (int k = 0; k < t.nlist; k++) c |= (il[k] == x); matched = (op == 6) ? c : !c; }
+            if (is_set) {                                                   // int64(float1) of amd64, not cvt.rzi's saturation
+                if (trunc(float1) == float1) { int64_t x = go_f2i64(float1); bool c = false; for (int k = 0; k < t.nlist; k++) c |= (il[k] == x); matched = (op == 6) ? c : !c; }
                 else matched = false;
                 return 0;
             }

@@ -12,6 +12,7 @@
 //   ClickHouse types   pkg/providers/clickhouse/columntypes/types.go:210-248, sink_table.go:196-235
 #pragma once
 #include <cerrno>
+#include <cmath>
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
@@ -242,7 +243,11 @@ private:
         if (t.kind == T_STR) { kind = LV_STRING; l.s = unquote(t.text); p_++; }
         else if (t.kind == T_DT) { kind = LV_TIME; l.i = parse_time_micro(t.text); p_++; }
         else if (kw(t, "TRUE") || kw(t, "FALSE")) { kind = LV_BOOL; l.i = upper(t.text) == "TRUE"; p_++; }
-        else if (t.kind == T_FLOAT) { kind = LV_FLOAT; l.f = strtod(t.text.c_str(), nullptr); p_++; }
+        else if (t.kind == T_FLOAT) {
+            kind = LV_FLOAT; l.f = strtod(t.text.c_str(), nullptr);
+            if (l.f == HUGE_VAL || l.f == -HUGE_VAL) throw FatalError(TF_E_FATAL_CONFIG, "filter: value out of range");   // strconv.ParseFloat: ErrRange (an underflow to 0 is not one)
+            p_++;
+        }
         else if (t.kind == T_INT) {
             kind = LV_INT; errno = 0; l.i = strtoll(t.text.c_str(), nullptr, 10);
             if (errno == ERANGE) throw FatalError(TF_E_FATAL_CONFIG, "filter: value out of range");
