@@ -165,7 +165,8 @@ typedef struct tf_batch {
 typedef struct tf_rowerr {
     uint32_t row;      /* index into the INPUT batch */
     uint16_t code;     /* TF_ROWERR_* */
-    uint16_t term;     /* index of the transformer in the plan that raised it; 0xff = raised before the chain (parser, host hand-off) */
+    uint16_t term;     /* index of the transformer in the plan that raised it, or the column (any index below 65536) for the codes documented
+                          "term = column"; 0xff = raised before the chain (parser, host hand-off) */
 } tf_rowerr;
 
 /* ---- wire formats for tfgpu_push_encode ----------------------------------- */

@@ -45,7 +45,7 @@ void box(const tf_col& c, uint64_t r, orc_val& v) {
     case TF_UINT16: v.kind = OG_UINT16; v.u = ((const uint16_t*)c.values)[r]; break;
     case TF_UINT32: v.kind = OG_UINT32; v.u = ((const uint32_t*)c.values)[r]; break;
     case TF_UINT64: v.kind = OG_UINT64; v.u = ((const uint64_t*)c.values)[r]; break;
-    case TF_FLOAT:  v.kind = OG_FLOAT32; v.f = ((const float*)c.values)[r]; break;
+    case TF_FLOAT:  v.kind = OG_FLOAT32; v.f = ((const float*)c.values)[r]; v.u = ((const uint32_t*)c.values)[r]; break;   // u: the bits (float -> double quiets a signaling NaN)
     case TF_DOUBLE: v.kind = OG_FLOAT64; v.f = ((const double*)c.values)[r]; break;
     case TF_BOOLEAN: v.kind = OG_BOOL; v.i = ((const uint8_t*)c.values)[r] != 0; break;
     case TF_INTERVAL: v.kind = OG_DURATION; v.i = ((const int64_t*)c.values)[r]; break;
@@ -325,7 +325,7 @@ bool append_value(ColBuilder& cb, const orc_val& v) {
     case TF_UINT32: { uint32_t x = is_null ? 0 : (uint32_t)v.u; cb.put(&x, 4); return true; }
     case TF_UINT64: { uint64_t x = is_null ? 0 : v.u; cb.put(&x, 8); return true; }
     case TF_BOOLEAN: { uint8_t x = is_null ? 0 : (v.i ? 1 : 0); cb.put(&x, 1); return true; }
-    case TF_FLOAT: { float x = is_null ? 0 : (float)v.f; cb.put(&x, 4); return true; }
+    case TF_FLOAT: { float x = is_null ? 0 : (float)v.f; if (!is_null && v.kind == OG_FLOAT32) std::memcpy(&x, &v.u, 4); cb.put(&x, 4); return true; }   // a Go float32 keeps its bits
     case TF_DOUBLE: { double x = is_null ? 0 : v.f; cb.put(&x, 8); return true; }
     case TF_DATE: {        // applyClickhouseDateBoundaries types.go:20-29, then Date = days since epoch (u16)
         int64_t s = is_null ? 0 : v.i;

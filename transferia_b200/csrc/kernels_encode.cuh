@@ -39,7 +39,7 @@ __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* total,
 // cast.ToInt64 / cast.ToUint64 of the value. One thread per row walks the loose columns in schema order, so the row's error is the first
 // failing column's, like Strictify's.
 struct StrictCol { const uint8_t* src; uint8_t* dst; const uint8_t* validity; int32_t src_tf, dst_tf, col, pad; };
-struct StrictArgs { const StrictCol* cols; int ncols; uint64_t nrows; uint8_t* err; uint8_t* term; };
+struct StrictArgs { const StrictCol* cols; int ncols; uint64_t nrows; uint8_t* err; uint16_t* term; };
 __device__ __forceinline__ int64_t go_f2i64(double f) { return (f >= -9223372036854775808.0 && f < 9223372036854775808.0) ? (int64_t)f : INT64_MIN; }   // CVTTSD2SQ
 __device__ __forceinline__ uint64_t go_f2u64(double f) { return f < 9223372036854775808.0 ? (uint64_t)go_f2i64(f) : ((uint64_t)go_f2i64(f - 9223372036854775808.0) ^ 0x8000000000000000ull); }
 #ifdef TF_KERNELS_ENCODE
@@ -85,9 +85,11 @@ __global__ void __launch_bounds__(256) k_strictify(StrictArgs a) {
         case TF_DOUBLE: ((double*)c.dst)[r] = cls == 0 ? (double)si : (cls == 1 ? (double)ui : f); break;                    // json.Number of the decimal text: the nearest float64
         default: c.dst[r] = cls == 2 ? (f != 0) : (cls == 1 ? ui != 0 : si != 0); break;                                     // TF_BOOLEAN: ToBoolE
         }
-        if (e && !err) { err = e; term = c.col < 0xff ? c.col : 0xfe; }
+        if (e && !err) { err = e; term = c.col; }
     }
-    if (err && !a.err[r]) { a.err[r] = (uint8_t)err; a.term[r] = (uint8_t)term; }
+    const bool mine = err && !a.err[r];                    // an error raised upstream (parser) keeps its code and term 0xff
+    if (mine) a.err[r] = (uint8_t)err;
+    a.term[r] = (uint16_t)(mine ? term : 0xff);
 }
 #endif  // TF_KERNELS_ENCODE
 
@@ -222,9 +224,9 @@ struct FilterArgs {
     const DFilterStep* steps; int nsteps;
     const uint32_t* expr_off;      // term ranges per expression (global expr index)
     const DTerm* terms; const uint8_t* blob;
-    uint8_t* keep; uint8_t* errcode; uint8_t* errstep; uint32_t* blockcnt; DState* st;
+    uint8_t* keep; uint8_t* errcode; uint16_t* errstep; uint32_t* blockcnt; DState* st;
     const uint8_t* pre_err;        // optional per-row error already raised upstream (parser): the row is dropped and reported
-    const uint8_t* pre_term;       // optional: the column an upstream error belongs to (Strictify), else the term is 0xff
+    const uint16_t* pre_term;      // optional: the column an upstream error belongs to (Strictify), else the term is 0xff
     int sink_guard;                // the rows go to a sink / serializer wire format that only takes INSERT rows here: update / delete rows that survive the chain are reported
 };
 
@@ -263,7 +265,7 @@ __global__ void __launch_bounds__(256) k_filter(FilterArgs a) {
         }
         if (keep && a.sink_guard && (kind == TF_KIND_UPDATE || kind == TF_KIND_DELETE)) { err = TF_ROWERR_SINK_KIND_HOST; estep = 0xff; keep = false; }
         a.keep[r] = keep ? 1 : 0;
-        a.errcode[r] = (uint8_t)err; a.errstep[r] = (uint8_t)estep; is_err = err != 0;
+        a.errcode[r] = (uint8_t)err; a.errstep[r] = (uint16_t)estep; is_err = err != 0;
     }
     const unsigned b = __ballot_sync(0xffffffffu, keep);
     const unsigned be = __ballot_sync(0xffffffffu, is_err);
@@ -277,7 +279,7 @@ __global__ void __launch_bounds__(256) k_filter(FilterArgs a) {
 // batch with a handful of failing rows does not ship its whole error-code arrays back.
 struct DevRowErr { uint32_t row; uint16_t code, term; };
 #ifdef TF_KERNELS_ENCODE
-__global__ void __launch_bounds__(256) k_collect_errors(const uint8_t* errcode, const uint8_t* errstep, uint64_t nrows, DevRowErr* out, unsigned long long* counter, unsigned long long cap) {
+__global__ void __launch_bounds__(256) k_collect_errors(const uint8_t* errcode, const uint16_t* errstep, uint64_t nrows, DevRowErr* out, unsigned long long* counter, unsigned long long cap) {
     const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const uint8_t c = r < nrows ? errcode[r] : 0;
     if (!c) return;

@@ -486,7 +486,7 @@ template <typename Sink> __device__ int dbz_row(Sink& s, const DCol* cols, const
 struct JsonArgs {
     const DCol* cols; const JsonCol* jcols; int njc; const uint8_t* names; const MaskKey* keys;
     const uint32_t* sel; DState* st; uint8_t* raw; uint32_t* row_size; uint32_t* tile_sum; const uint64_t* tile_base; const uint64_t* col_bytes;
-    int mode; uint32_t flags; uint8_t* errcode; uint8_t* errstep;      // mode 0 ClickHouse JSONEachRow, 1 serializer JSON, 2 serializer CSV, 3 Debezium messages
+    int mode; uint32_t flags; uint8_t* errcode; uint16_t* errstep;     // mode 0 ClickHouse JSONEachRow, 1 serializer JSON, 2 serializer CSV, 3 Debezium messages
     DbzEmitArgs dz;
 };
 
@@ -509,7 +509,7 @@ __global__ void __launch_bounds__(TF_JSON_TILE) k_json_sizes(JsonArgs a) {
     if (j < n) {
         const uint64_t r = a.sel ? a.sel[j] : j; CountSink cs; cs.n = 0;
         const int bad = json_any_row(cs, a, r, j, true); sz = cs.n; a.row_size[j] = sz;
-        if (bad >= 0) { a.errcode[r] = TF_ROWERR_SER_VALUE; a.errstep[r] = (uint8_t)bad; atomicAdd((unsigned long long*)&a.st->n_errors, 1ull); }
+        if (bad >= 0) { a.errcode[r] = TF_ROWERR_SER_VALUE; a.errstep[r] = (uint16_t)bad; atomicAdd((unsigned long long*)&a.st->n_errors, 1ull); }
     }
     uint32_t tot; block_excl_scan(sz, &tot, sm);
     if (threadIdx.x == 0) a.tile_sum[blockIdx.x] = tot;

@@ -16,7 +16,7 @@ namespace tfk {
 void launch_k_strictify(dim3 grid, dim3 block, size_t smem, cudaStream_t s, StrictArgs a);
 void launch_k_filter(dim3 grid, dim3 block, size_t smem, cudaStream_t s, FilterArgs a);
 void launch_k_scan_blockcnt(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint32_t* blockcnt, uint32_t* blockoff, uint32_t nblocks, DState* st);
-void launch_k_collect_errors(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint8_t* errcode, const uint8_t* errstep, uint64_t nrows, DevRowErr* out, unsigned long long* counter, unsigned long long cap);
+void launch_k_collect_errors(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint8_t* errcode, const uint16_t* errstep, uint64_t nrows, DevRowErr* out, unsigned long long* counter, unsigned long long cap);
 void launch_k_compact_sel(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint8_t* keep, const uint32_t* blockoff, uint64_t nrows, uint32_t* sel);
 void launch_k_layout_scan(dim3 grid, dim3 block, size_t smem, cudaStream_t s, LayoutArgs a);
 void launch_k_layout_finish(dim3 grid, dim3 block, size_t smem, cudaStream_t s, LayoutArgs a);

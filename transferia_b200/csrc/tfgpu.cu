@@ -91,7 +91,7 @@ struct tfgpu_engine {
     DState* d_state = nullptr; DCol* d_cols = nullptr; size_t d_cols_cap = 0;
     int32_t* d_call_slots = nullptr; ColRegions* d_regions = nullptr; size_t d_call_cap = 0;   // columnar mode, per call
     // pointers into `work` for the last call
-    uint8_t *keep = nullptr, *errcode = nullptr, *errstep = nullptr; uint32_t *blockcnt = nullptr, *blockoff = nullptr, *sel = nullptr;
+    uint8_t *keep = nullptr, *errcode = nullptr; uint16_t* errstep = nullptr; uint32_t *blockcnt = nullptr, *blockoff = nullptr, *sel = nullptr;
     uint32_t* tile_sum = nullptr; uint64_t* tile_base = nullptr; uint64_t* col_bytes = nullptr; uint32_t* comp_size = nullptr; uint64_t* wire_off = nullptr; unsigned long long* frame_pfx = nullptr;
     uint64_t last_nrows = 0; bool last_has_filter = false, last_has_sharder = false; int last_wire_fmt = 0;
     uint8_t* pinned = nullptr; size_t pinned_cap = 0;
@@ -219,7 +219,7 @@ void upload_plan(PlanDev& pd) {
         if (nullable && kind == OK_TODT) pd.fixed_slots.push_back((int32_t)c | TF_SLOT_ZEROMAP);
         else if (nullable && kind != OK_MASK && kind != OK_TOSTR) pd.fixed_slots.push_back((int32_t)c | TF_SLOT_NULLMAP);
     }
-    if (pd.str_slots.size() > 256) throw tfplan::FatalError(TF_E_FATAL_UNSUPPORTED, "more than 256 String columns");
+    if (pd.str_slots.size() > 65535) throw tfplan::FatalError(TF_E_FATAL_UNSUPPORTED, "more than 65535 String columns (one grid row per column)");
     // JSONEachRow descriptors: column name + the ClickHouse class of the RESULT type (columntypes.ToChType)
     std::vector<JsonCol> jcols; std::vector<uint8_t> jnames;
     for (size_t k = 0; k < pl.out_cols.size(); k++) {
@@ -392,12 +392,12 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
     // work arena
     const size_t nslot_alloc = (size_t)(pd.n_str > 0 ? pd.n_str : 1);
     Layout W;
-    const size_t o_keep = W.take(n), o_errcode = W.take(n), o_errstep = W.take(n), o_blockcnt = W.take(sz.nblocks * 4), o_blockoff = W.take(sz.nblocks * 4),
+    const size_t o_keep = W.take(n), o_errcode = W.take(n), o_errstep = W.take(2 * n), o_blockcnt = W.take(sz.nblocks * 4), o_blockoff = W.take(sz.nblocks * 4),
                  o_sel = W.take(n * 4), o_tile_sum = W.take(nslot_alloc * sz.ntiles_cap * 4), o_tile_base = W.take(nslot_alloc * sz.ntiles_cap * 8),
-                 o_comp = W.take(sz.n_frames_max * 4), o_wire_off = W.take(sz.n_frames_max * 8), o_pfx = W.take(sz.n_frames_max * 8), o_col_bytes = W.take(256 * 8);
+                 o_comp = W.take(sz.n_frames_max * 4), o_wire_off = W.take(sz.n_frames_max * 8), o_pfx = W.take(sz.n_frames_max * 8), o_col_bytes = W.take(nslot_alloc * 8);
     e->work.ensure(W.total());
     uint8_t* w = e->work.p;
-    e->keep = w + o_keep; e->errcode = w + o_errcode; e->errstep = w + o_errstep;
+    e->keep = w + o_keep; e->errcode = w + o_errcode; e->errstep = (uint16_t*)(w + o_errstep);
     e->blockcnt = (uint32_t*)(w + o_blockcnt); e->blockoff = (uint32_t*)(w + o_blockoff); e->sel = (uint32_t*)(w + o_sel);
     e->tile_sum = (uint32_t*)(w + o_tile_sum); e->tile_base = (uint64_t*)(w + o_tile_base);
     e->comp_size = (uint32_t*)(w + o_comp); e->wire_off = (uint64_t*)(w + o_wire_off); e->frame_pfx = (unsigned long long*)(w + o_pfx); e->col_bytes = (uint64_t*)(w + o_col_bytes);
@@ -428,10 +428,10 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
         }
     }
     if (!pre_err) e->prof_n = 0;
-    const uint8_t* pre_term = nullptr;
+    const uint16_t* pre_term = nullptr;
     if (!strict.empty() && n) {        // Strictify pre-pass: loose fixed-width values -> the schema's type, range / cast failures as row errors
         Layout S;
-        const size_t o_desc = S.take(strict.size() * sizeof(StrictCol)), o_err = S.take(n), o_term = S.take(n);
+        const size_t o_desc = S.take(strict.size() * sizeof(StrictCol)), o_err = S.take(n), o_term = S.take(2 * n);
         std::vector<size_t> o_val(strict.size());
         for (size_t k = 0; k < strict.size(); k++) o_val[k] = S.take((size_t)in_width(strict[k].dst_tf) * n + 16);
         e->strict_stage.ensure(S.total() + 256);
@@ -439,10 +439,9 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
         for (size_t k = 0; k < strict.size(); k++) { strict[k].dst = B + o_val[k]; hc[strict[k].col].values = B + o_val[k]; }
         CK(cudaMemcpyAsync(B + o_desc, strict.data(), strict.size() * sizeof(StrictCol), cudaMemcpyHostToDevice, s));
         if (pre_err) CK(cudaMemcpyAsync(B + o_err, pre_err, n, cudaMemcpyDeviceToDevice, s)); else CK(cudaMemsetAsync(B + o_err, 0, n, s));
-        CK(cudaMemsetAsync(B + o_term, 0xff, n, s));
-        StrictArgs sa{(const StrictCol*)(B + o_desc), (int)strict.size(), n, B + o_err, B + o_term};
+        StrictArgs sa{(const StrictCol*)(B + o_desc), (int)strict.size(), n, B + o_err, (uint16_t*)(B + o_term)};
         e->prof_begin("k_strictify", s); launch_k_strictify((uint32_t)((n + 255) / 256), 256, 0, s, sa); e->prof_end(s);
-        pre_err = B + o_err; pre_term = B + o_term;
+        pre_err = B + o_err; pre_term = (const uint16_t*)(B + o_term);
     }
     CK(cudaMemcpyAsync(e->d_cols, hc.data(), sizeof(DCol) * nc, cudaMemcpyHostToDevice, s));
     CK(cudaMemsetAsync(e->d_state, 0, sizeof(DState), s));
@@ -501,7 +500,7 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
                     (uint32_t*)e->work_json_sizes(n), e->tile_sum, e->tile_base, e->col_bytes,
                     dbz ? 3 : ser ? (wire_base == TF_WIRE_SER_JSON ? 1 : 2) : 0, (uint32_t)(((wire_fmt & TF_WIRE_F_CLOSING_NEWLINE) ? TF_SER_NL : 0) | ((wire_fmt & TF_WIRE_F_ANY_AS_STRING) ? TF_SER_AAS : 0)), e->errcode, e->errstep, DbzEmitArgs{}};
         if (dbz) { ja.jcols = pd.d_sjcols; e->dbz_keysz.ensure(n * 4 + 256); e->dbz_msgsz.ensure(n * 28 + 256); ja.dz = e->dbz; ja.dz.key_size = (uint32_t*)e->dbz_keysz.p; ja.dz.msg_size = (uint32_t*)e->dbz_msgsz.p; }
-        if (ser && !has_filter && n) { CK(cudaMemsetAsync(e->errcode, 0, n, s)); CK(cudaMemsetAsync(e->errstep, 0, n, s)); }
+        if (ser && !has_filter && n) { CK(cudaMemsetAsync(e->errcode, 0, n, s)); CK(cudaMemsetAsync(e->errstep, 0, 2 * n, s)); }
         if (jt) { e->prof_begin("k_json_sizes", s); launch_k_json_sizes(jt, TF_JSON_TILE, 0, s, ja); e->prof_end(s); }
         LayoutArgs lj{e->d_cols, 0, pd.d_out_cols, pd.d_str_slots, 1, e->tile_sum, e->tile_base, sz.ntiles_cap, pd.d_col_headers, pd.d_col_header_off,
                       e->raw.p, e->d_state, n, 1, e->frame_bytes, e->col_bytes};
@@ -799,16 +798,16 @@ int tfgpu_push_encode_selective(tfgpu_engine* e, int plan_id, int wire_fmt, cons
         CK(cudaMemsetAsync(e->d_state, 0, sizeof(DState), s));
         const uint32_t nb = (uint32_t)((n + 255) / 256);
         Layout L;
-        const size_t o_flags = L.take(3 * n), o_blockcnt = L.take((size_t)nb * 4);     // keep, errcode, errstep back to back: one copy to the host
+        const size_t o_flags = L.take(4 * n), o_blockcnt = L.take((size_t)nb * 4);     // keep, errcode, errstep (u16) back to back: one copy to the host
         e->sel_stage.ensure(L.total() + 256);
         uint8_t* B = e->sel_stage.p + o_flags;
-        FilterArgs fa{e->d_cols, dev_kinds, n, pd.d_fsteps, pd.n_fsteps, pd.d_expr_off, pd.d_terms, pd.d_blob, B, B + n, B + 2 * n, (uint32_t*)(e->sel_stage.p + o_blockcnt), e->d_state, nullptr, nullptr, 0};
+        FilterArgs fa{e->d_cols, dev_kinds, n, pd.d_fsteps, pd.n_fsteps, pd.d_expr_off, pd.d_terms, pd.d_blob, B, B + n, (uint16_t*)(B + 2 * n), (uint32_t*)(e->sel_stage.p + o_blockcnt), e->d_state, nullptr, nullptr, 0};
         e->prof_n = 0;
         e->prof_begin("k_filter", s); launch_k_filter(nb, 256, 0, s, fa); e->prof_end(s);
-        if (e->sel_host_cap < 3 * n) { if (e->sel_host) CK(cudaFreeHost(e->sel_host)); e->sel_host = nullptr; e->sel_host_cap = 0; const size_t want = align_up(3 * n + 3 * n / 4 + 4096, 1 << 16); CK(cudaMallocHost(&e->sel_host, want)); e->sel_host_cap = want; }
-        CK(cudaMemcpyAsync(e->sel_host, B, 3 * n, cudaMemcpyDeviceToHost, s));
+        if (e->sel_host_cap < 4 * n) { if (e->sel_host) CK(cudaFreeHost(e->sel_host)); e->sel_host = nullptr; e->sel_host_cap = 0; const size_t want = align_up(4 * n + n + 4096, 1 << 16); CK(cudaMallocHost(&e->sel_host, want)); e->sel_host_cap = want; }
+        CK(cudaMemcpyAsync(e->sel_host, B, 4 * n, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
-        const uint8_t* keep = e->sel_host; const uint8_t* ecode = keep + n; const uint8_t* estep = keep + 2 * n;
+        const uint8_t* keep = e->sel_host; const uint8_t* ecode = keep + n; const uint16_t* estep = (const uint16_t*)(keep + 2 * n);
         const auto t_1 = std::chrono::steady_clock::now();
         // ---- host gather of the kept rows
         if (!e->gather_pool) { const int rc = tfgpu_columnar_create(&e->gather_pool); if (rc) return fail(e, rc, "cannot create the gather pool"); }
