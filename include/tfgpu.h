@@ -456,8 +456,10 @@ void tfgpu_deflate_stream_free(tfgpu_deflate_stream* s);
 /* Number of kernel launches issued by this engine since creation (bench `gpu_launches`). */
 uint64_t tfgpu_engine_launch_count(const tfgpu_engine* e);
 
-/* Optional per-kernel timing of the LAST call with CUDA events on the engine's stream (bench.py roofline).
- * tfgpu_profile_read synchronises the stream and returns JSON [{"name":"k_lz4_frames","ms":..},..] owned by the engine. */
+/* Optional per-kernel timing with CUDA events on the streams the kernels run on (bench.py roofline): the profile holds every launch,
+ * in launch order, of the last call that launched a kernel after tfgpu_profile_enable; calls that launch none (tfgpu_resident_stats,
+ * tfgpu_profile_read itself) leave it as it is. tfgpu_profile_read synchronises the stream and returns JSON
+ * [{"name":"k_lz4_frames","ms":..},..] owned by the engine. */
 int tfgpu_profile_enable(tfgpu_engine* e, int on);
 const char* tfgpu_profile_read(tfgpu_engine* e);
 

@@ -55,6 +55,7 @@ struct CsvArgs {
 // `endbits` (JSON parser): bit p set = byte p is the last byte of a message, which ends a line like '\n' does
 __device__ __forceinline__ bool csv_line_end(const uint8_t* text, const uint32_t* endbits, uint64_t p) { return text[p] == '\n' || (endbits && ((endbits[p >> 5] >> (p & 31)) & 1)); }
 
+__global__ void k_csv_count_nl(const uint8_t* text, uint64_t len, uint32_t* blk_cnt, const uint32_t* endbits);
 #ifdef TF_KERNELS_CSV
 __global__ void __launch_bounds__(256) k_csv_count_nl(const uint8_t* text, uint64_t len, uint32_t* blk_cnt, const uint32_t* endbits) {
     __shared__ uint32_t sm[33];
@@ -66,6 +67,7 @@ __global__ void __launch_bounds__(256) k_csv_count_nl(const uint8_t* text, uint6
 }
 #endif  // TF_KERNELS_CSV
 
+__global__ void k_csv_line_index(const uint8_t* text, uint64_t len, const uint32_t* blk_off, uint32_t* line_end, const uint32_t* endbits);
 #ifdef TF_KERNELS_CSV
 __global__ void __launch_bounds__(256) k_csv_line_index(const uint8_t* text, uint64_t len, const uint32_t* blk_off, uint32_t* line_end, const uint32_t* endbits) {
     __shared__ uint32_t sm[33];
@@ -82,6 +84,7 @@ __global__ void __launch_bounds__(256) k_csv_line_index(const uint8_t* text, uin
 // Var-width columns may arrive with uint8 / uint16 LENGTHS instead of uint32 offsets (tf_col.flags TF_COL_LENS8 / 16: a quarter / half
 // of the offset bytes over PCIe); widened here, then scanned into offsets by the three kernels above.
 struct LensSrc { const uint8_t* p; int32_t width, pad; };
+__global__ void k_widen_lens(const LensSrc* src, uint64_t nrows, uint32_t* out);
 #ifdef TF_KERNELS_CSV
 __global__ void __launch_bounds__(256) k_widen_lens(const LensSrc* src, uint64_t nrows, uint32_t* out /* [nslots][nrows] */) {
     const LensSrc ls = src[blockIdx.y];
@@ -471,6 +474,7 @@ static __device__ void csv_rows_by_warp(const CsvArgs& a, uint64_t row0, uint64_
 #define CSV_TILE_ROWS 32
 #define CSV_TILE_BYTES 28672
 #define CSV_TF 250            /* element boundaries kept per line */
+__global__ void k_csv_pass1(CsvArgs a);
 #ifdef TF_KERNELS_CSV
 __global__ void __launch_bounds__(32 * CSV_WARPS, 4) k_csv_pass1(CsvArgs a) {
     __shared__ __align__(16) uint8_t s_tile[CSV_TILE_BYTES + 16];      // (the warp-per-line tables alias it)
@@ -606,6 +610,7 @@ __global__ void __launch_bounds__(32 * CSV_WARPS, 4) k_csv_pass1(CsvArgs a) {
 #endif  // TF_KERNELS_CSV
 
 // per text column: offsets[r] = sum of lengths of rows < r. One CTA per column walks its rows in chunks.
+__global__ void k_csv_offsets(const uint32_t* span_len, uint64_t nrows, uint32_t* offsets, uint64_t* col_total);
 #ifdef TF_KERNELS_CSV
 __global__ void __launch_bounds__(1024) k_csv_offsets(const uint32_t* span_len, uint64_t nrows, uint32_t* offsets /* [nslots][nrows+1] */, uint64_t* col_total) {
     __shared__ uint32_t sm[33];
@@ -625,6 +630,7 @@ __global__ void __launch_bounds__(1024) k_csv_offsets(const uint32_t* span_len, 
 // The same scan over many CTAs: chunk sums, a scan of the chunk sums per column, then the offsets (3 short launches instead
 // of one CTA per column walking every row).
 #define CSV_OFF_CHUNK 4096
+__global__ void k_offsets_sum(const uint32_t* span_len, uint64_t nrows, uint32_t nchunks, uint64_t* chunk_sum);
 #ifdef TF_KERNELS_CSV
 __global__ void __launch_bounds__(1024) k_offsets_sum(const uint32_t* span_len, uint64_t nrows, uint32_t nchunks, uint64_t* chunk_sum /* [nslots][nchunks] */) {
     __shared__ uint32_t sm[33];
@@ -637,6 +643,7 @@ __global__ void __launch_bounds__(1024) k_offsets_sum(const uint32_t* span_len, 
     if (threadIdx.x == 0) chunk_sum[(size_t)blockIdx.y * nchunks + blockIdx.x] = tot;
 }
 #endif  // TF_KERNELS_CSV
+__global__ void k_offsets_chunks(uint64_t* chunk_sum, uint32_t nchunks, uint64_t* col_total);
 #ifdef TF_KERNELS_CSV
 __global__ void __launch_bounds__(32) k_offsets_chunks(uint64_t* chunk_sum, uint32_t nchunks, uint64_t* col_total) {     // in place: exclusive scan per column, one warp
     uint64_t* cs = chunk_sum + (size_t)blockIdx.x * nchunks;
@@ -654,6 +661,7 @@ __global__ void __launch_bounds__(32) k_offsets_chunks(uint64_t* chunk_sum, uint
     if (lane == 0) col_total[blockIdx.x] = carry;
 }
 #endif  // TF_KERNELS_CSV
+__global__ void k_offsets_write(const uint32_t* span_len, uint64_t nrows, uint32_t nchunks, const uint64_t* chunk_base, const uint64_t* col_total, uint32_t* offsets);
 #ifdef TF_KERNELS_CSV
 __global__ void __launch_bounds__(1024) k_offsets_write(const uint32_t* span_len, uint64_t nrows, uint32_t nchunks, const uint64_t* chunk_base, const uint64_t* col_total, uint32_t* offsets /* [nslots][nrows+1] */) {
     __shared__ uint32_t sm[33];
@@ -673,6 +681,7 @@ __global__ void __launch_bounds__(1024) k_offsets_write(const uint32_t* span_len
 struct CsvCopyArgs { const uint8_t* text; const uint32_t* span_start; const uint32_t* span_len; const uint32_t* span_raw; const uint32_t* offsets; uint8_t* heap;
                      const uint64_t* col_base; uint64_t nrows; uint8_t quote; };      // a doubled quote character in a flagged span is copied as one '"' (swapToSingleQuotes)
 
+__global__ void k_csv_pass2(CsvCopyArgs a);
 #ifdef TF_KERNELS_CSV
 __global__ void __launch_bounds__(256) k_csv_pass2(CsvCopyArgs a) {
     const uint64_t row = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;

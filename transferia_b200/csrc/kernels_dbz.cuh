@@ -271,6 +271,7 @@ __device__ __forceinline__ const uint8_t* dbz_stage_span(const DbzArgs& a, uint8
     return stage - lo16;
 }
 
+__global__ void k_dbz_pass1(DbzArgs a);
 #ifdef TF_KERNELS_DBZ
 __global__ void __launch_bounds__(128) k_dbz_pass1(DbzArgs a) {
     extern __shared__ __align__(16) uint8_t dbz_stage[];
@@ -437,6 +438,7 @@ __global__ void __launch_bounds__(128) k_dbz_pass1(DbzArgs a) {
 
 struct DbzWriteArgs { DbzArgs a; const uint32_t* offsets; uint8_t* heap; const uint64_t* col_base; };
 
+__global__ void k_dbz_pass2(DbzWriteArgs w);
 #ifdef TF_KERNELS_DBZ
 __global__ void __launch_bounds__(128) k_dbz_pass2(DbzWriteArgs w) {
     const DbzArgs& a = w.a;

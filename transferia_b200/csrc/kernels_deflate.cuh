@@ -61,6 +61,8 @@ struct DeflateArgs {
     int zlib;                                // 0 gzip, 1 zlib
     DState* st;                              // wire_total
 };
+__global__ void k_deflate_chunks(DeflateArgs a);
+__global__ void k_deflate_finish(DeflateArgs a);
 
 __device__ __forceinline__ uint32_t df_ld32(const uint32_t* w, uint32_t p) {   // 4 bytes at byte offset p of the chunk
     const uint32_t i = p >> 2, s = (p & 3) * 8;

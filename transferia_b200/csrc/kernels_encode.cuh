@@ -42,6 +42,7 @@ struct StrictCol { const uint8_t* src; uint8_t* dst; const uint8_t* validity; in
 struct StrictArgs { const StrictCol* cols; int ncols; uint64_t nrows; uint8_t* err; uint16_t* term; };
 __device__ __forceinline__ int64_t go_f2i64(double f) { return (f >= -9223372036854775808.0 && f < 9223372036854775808.0) ? (int64_t)f : INT64_MIN; }   // CVTTSD2SQ
 __device__ __forceinline__ uint64_t go_f2u64(double f) { return f < 9223372036854775808.0 ? (uint64_t)go_f2i64(f) : ((uint64_t)go_f2i64(f - 9223372036854775808.0) ^ 0x8000000000000000ull); }
+__global__ void k_strictify(StrictArgs a);
 #ifdef TF_KERNELS_ENCODE
 __global__ void __launch_bounds__(256) k_strictify(StrictArgs a) {
     const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -231,6 +232,7 @@ struct FilterArgs {
 };
 
 // FilterRowsTransformer.Apply (filter_rows.go:99-130): one thread per row.
+__global__ void k_filter(FilterArgs a);
 #ifdef TF_KERNELS_ENCODE
 __global__ void __launch_bounds__(256) k_filter(FilterArgs a) {
     __shared__ uint32_t s_cnt, s_err;
@@ -278,6 +280,7 @@ __global__ void __launch_bounds__(256) k_filter(FilterArgs a) {
 // The rows that raised an error as (row, code, term) triples: appended through a counter (the host sorts the few it gets by row), so a
 // batch with a handful of failing rows does not ship its whole error-code arrays back.
 struct DevRowErr { uint32_t row; uint16_t code, term; };
+__global__ void k_collect_errors(const uint8_t* errcode, const uint16_t* errstep, uint64_t nrows, DevRowErr* out, unsigned long long* counter, unsigned long long cap);
 #ifdef TF_KERNELS_ENCODE
 __global__ void __launch_bounds__(256) k_collect_errors(const uint8_t* errcode, const uint16_t* errstep, uint64_t nrows, DevRowErr* out, unsigned long long* counter, unsigned long long cap) {
     const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -289,6 +292,7 @@ __global__ void __launch_bounds__(256) k_collect_errors(const uint8_t* errcode, 
 #endif  // TF_KERNELS_ENCODE
 
 // exclusive scan of per-block kept counts (single block), total -> state.n_kept
+__global__ void k_scan_blockcnt(const uint32_t* blockcnt, uint32_t* blockoff, uint32_t nblocks, DState* st);
 #ifdef TF_KERNELS_ENCODE
 __global__ void __launch_bounds__(1024) k_scan_blockcnt(const uint32_t* blockcnt, uint32_t* blockoff, uint32_t nblocks, DState* st) {
     __shared__ uint32_t sm[33];
@@ -305,6 +309,7 @@ __global__ void __launch_bounds__(1024) k_scan_blockcnt(const uint32_t* blockcnt
 #endif  // TF_KERNELS_ENCODE
 
 // sel[j] = index of the j-th kept row (order preserved)
+__global__ void k_compact_sel(const uint8_t* keep, const uint32_t* blockoff, uint64_t nrows, uint32_t* sel);
 #ifdef TF_KERNELS_ENCODE
 __global__ void __launch_bounds__(256) k_compact_sel(const uint8_t* keep, const uint32_t* blockoff, uint64_t nrows, uint32_t* sel) {
     __shared__ uint32_t sm[33];
@@ -338,6 +343,7 @@ struct LayoutArgs {
 // Block layout (clickhouse-go/v2 v2.46.0 lib/proto/block.go, revision 54460):
 //   uvarint 1, u8 is_overflows=0, uvarint 2, i32 bucket_num=-1, uvarint 0, uvarint ncols, uvarint nrows,
 //   per column: string name, string type, u8 custom_serialization=0, [null map], data
+__global__ void k_layout_scan(LayoutArgs a);
 #ifdef TF_KERNELS_ENCODE
 __global__ void __launch_bounds__(1024) k_layout_scan(LayoutArgs a) {
     __shared__ uint32_t sm[33];
@@ -356,6 +362,7 @@ __global__ void __launch_bounds__(1024) k_layout_scan(LayoutArgs a) {
 }
 #endif  // TF_KERNELS_ENCODE
 
+__global__ void k_layout_finish(LayoutArgs a);
 #ifdef TF_KERNELS_ENCODE
 __global__ void __launch_bounds__(256) k_layout_finish(LayoutArgs a) {
     __shared__ uint64_t s_size[3][256];     // header, null map, data bytes per column (ncols <= 256 per pass)
@@ -407,6 +414,7 @@ __global__ void __launch_bounds__(256) k_layout_finish(LayoutArgs a) {
 // [values | validity bitmap | aux | offsets | heap]; the region table goes back to the host with the data.
 struct ColRegions { uint64_t values, validity, aux, offsets, heap, heap_len; };   // offsets into the buffer; ~0 = absent
 
+__global__ void k_layout_columnar(LayoutArgs a, ColRegions* regions);
 #ifdef TF_KERNELS_ENCODE
 __global__ void __launch_bounds__(256) k_layout_columnar(LayoutArgs a, ColRegions* regions) {
     __shared__ uint64_t s_sz[5][256];
@@ -551,6 +559,7 @@ template <int K, int INW, int W> __device__ __forceinline__ void encode_stream(c
 }
 
 // Fixed-width columns, null maps and (columnar output) aux arrays: blockIdx.y = stream slot.
+__global__ void k_encode_fixed(EncodeArgs a);
 #ifdef TF_KERNELS_ENCODE
 __global__ void __launch_bounds__(256) k_encode_fixed(EncodeArgs a) {
     const int32_t slot = a.slots[blockIdx.y];
@@ -580,6 +589,7 @@ __global__ void __launch_bounds__(256) k_encode_fixed(EncodeArgs a) {
 #endif  // TF_KERNELS_ENCODE
 
 // validity bitmap of the kept rows: one thread per output byte (8 rows)
+__global__ void k_pack_validity(EncodeArgs a);
 #ifdef TF_KERNELS_ENCODE
 __global__ void __launch_bounds__(256) k_pack_validity(EncodeArgs a) {
     const DCol c = a.cols[a.slots[blockIdx.y]];
@@ -606,6 +616,7 @@ __global__ void __launch_bounds__(256) k_pack_validity(EncodeArgs a) {
 // JSON text in a string -- an estimate, flagged in DESIGN.md.
 struct MeasureArgs { const DCol* cols; int ncols; uint64_t nrows; uint64_t* per_row; unsigned long long* total; };
 
+__global__ void k_measure(MeasureArgs a);
 #ifdef TF_KERNELS_ENCODE
 __global__ void __launch_bounds__(256) k_measure(MeasureArgs a) {
     __shared__ uint32_t sm[33];

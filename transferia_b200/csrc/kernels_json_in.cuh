@@ -49,6 +49,7 @@ struct JsnArgs {
 };
 
 // ------------------------------------------------------------------ line helpers
+__global__ void k_json_mark_msgs(const uint64_t* msg_end, uint32_t nmsgs, uint32_t* bits);
 #ifdef TF_KERNELS_JSON_IN
 __global__ void __launch_bounds__(256) k_json_mark_msgs(const uint64_t* msg_end, uint32_t nmsgs, uint32_t* bits) {
     const uint32_t m = blockIdx.x * blockDim.x + threadIdx.x;
@@ -63,6 +64,7 @@ __device__ __forceinline__ void jsn_line(const uint8_t* text, const uint32_t* li
     if (le > ls && text[le - 1] == '\r') le--;            // bufio.ScanLines dropCR
     n = le - ls;
 }
+__global__ void k_json_count_nonempty(const uint8_t* text, const uint32_t* line_end, uint64_t nlines, uint32_t* blk_cnt);
 #ifdef TF_KERNELS_JSON_IN
 __global__ void __launch_bounds__(128) k_json_count_nonempty(const uint8_t* text, const uint32_t* line_end, uint64_t nlines, uint32_t* blk_cnt) {
     __shared__ uint32_t sm[33];
@@ -72,6 +74,7 @@ __global__ void __launch_bounds__(128) k_json_count_nonempty(const uint8_t* text
     if (threadIdx.x == 0) blk_cnt[blockIdx.x] = tot;
 }
 #endif  // TF_KERNELS_JSON_IN
+__global__ void k_json_rank(const uint8_t* text, const uint32_t* line_end, uint64_t nlines, const uint32_t* blk_off, uint32_t* rank);
 #ifdef TF_KERNELS_JSON_IN
 __global__ void __launch_bounds__(128) k_json_rank(const uint8_t* text, const uint32_t* line_end, uint64_t nlines, const uint32_t* blk_off, uint32_t* rank) {
     __shared__ uint32_t sm[33];
@@ -82,6 +85,7 @@ __global__ void __launch_bounds__(128) k_json_rank(const uint8_t* text, const ui
 }
 #endif  // TF_KERNELS_JSON_IN
 // rank of the first line of every message: _idx counts the non-empty lines of its own message from 1 (:526-531)
+__global__ void k_json_msg_first(const uint64_t* msg_end, uint32_t nmsgs, const uint32_t* line_end, uint64_t nlines, const uint32_t* rank, uint32_t* msg_rank0);
 #ifdef TF_KERNELS_JSON_IN
 __global__ void __launch_bounds__(256) k_json_msg_first(const uint64_t* msg_end, uint32_t nmsgs, const uint32_t* line_end, uint64_t nlines, const uint32_t* rank, uint32_t* msg_rank0) {
     const uint32_t m = blockIdx.x * blockDim.x + threadIdx.x;
@@ -724,6 +728,7 @@ __device__ __forceinline__ const uint8_t* jsn_stage_span(const JsnArgs& a, uint8
 }
 
 // ------------------------------------------------------------------ pass 1
+__global__ void k_json_pass1(JsnArgs a);
 #ifdef TF_KERNELS_JSON_IN
 __global__ void __launch_bounds__(128) k_json_pass1(JsnArgs a) {
     extern __shared__ __align__(16) uint8_t jsn_stage[];
@@ -809,6 +814,7 @@ __global__ void __launch_bounds__(128) k_json_pass1(JsnArgs a) {
 // ------------------------------------------------------------------ pass 2: text cells
 struct JsnWriteArgs { JsnArgs a; const uint32_t* offsets; uint8_t* heap; const uint64_t* col_base; };
 
+__global__ void k_json_pass2(JsnWriteArgs w);
 #ifdef TF_KERNELS_JSON_IN
 __global__ void __launch_bounds__(128) k_json_pass2(JsnWriteArgs w) {
     extern __shared__ __align__(16) uint8_t jsn_stage[];

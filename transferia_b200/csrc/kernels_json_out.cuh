@@ -499,6 +499,7 @@ template <typename Sink> __device__ __forceinline__ int json_any_row(Sink& s, co
 
 #define TF_JSON_TILE 256
 
+__global__ void k_json_sizes(JsonArgs a);
 #ifdef TF_KERNELS_JSON_OUT
 __global__ void __launch_bounds__(TF_JSON_TILE) k_json_sizes(JsonArgs a) {
     __shared__ uint32_t sm[33];
@@ -516,6 +517,7 @@ __global__ void __launch_bounds__(TF_JSON_TILE) k_json_sizes(JsonArgs a) {
 }
 #endif  // TF_KERNELS_JSON_OUT
 
+__global__ void k_json_write(JsonArgs a);
 #ifdef TF_KERNELS_JSON_OUT
 __global__ void __launch_bounds__(TF_JSON_TILE) k_json_write(JsonArgs a) {
     __shared__ uint32_t sm[33];

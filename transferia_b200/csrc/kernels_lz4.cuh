@@ -70,6 +70,7 @@ struct Lz4Args {
     uint32_t frame_bytes;
     unsigned long long* phases;     // optional [8]: cycles thread 0 of every CTA spent per phase (tfgpu_debug_lz4_phases), NULL = off
 };
+__global__ void k_lz4_frames(Lz4Args a);
 #define LZ_PHASE(k) do { if (a.phases && tid == 0) { const long long t_ = clock64(); atomicAdd(&a.phases[k], (unsigned long long)(t_ - t_ph)); t_ph = t_; } } while (0)
 
 __device__ __forceinline__ uint32_t ld32u(const uint32_t* w, uint32_t p) {   // 4 bytes at byte offset p of the frame in shared memory
@@ -628,6 +629,7 @@ __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
 
+__global__ void k_frame_seal(FrameArgs a);
 #ifdef TF_KERNELS_LZ4
 __global__ void __launch_bounds__(32) k_frame_seal(FrameArgs a) {
     extern __shared__ __align__(16) uint8_t seal_smem[];

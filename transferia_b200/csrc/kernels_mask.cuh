@@ -132,6 +132,7 @@ __device__ inline void mask_digest_hex(const DCol& c, uint64_t r, const MaskKey&
 }
 
 // one thread per (kept row, masked column): "\x40" + 64 hex chars into the block (or the bare digest, columnar output)
+__global__ void k_mask_encode(MaskArgs a);
 #ifdef TF_KERNELS_MASK
 __global__ void __launch_bounds__(128) k_mask_encode(MaskArgs a) {
     const DCol c = a.cols[a.slots[blockIdx.y]];
@@ -160,6 +161,7 @@ struct ShardCol { int32_t col, form, pad0, pad1; };       // form: 0 text of the
 struct ShardArgs { const DCol* cols; const ShardCol* sc; int nsc; const MaskKey* keys; const uint32_t* sel; DState* st; uint32_t shards; uint32_t* part; };
 struct CrcSink { uint32_t c; const uint32_t* tab; __device__ __forceinline__ void put(uint8_t b) { c = tab[(c ^ b) & 0xffu] ^ (c >> 8); } };
 
+__global__ void k_shard_ids(ShardArgs a);
 #ifdef TF_KERNELS_MASK
 __global__ void __launch_bounds__(256) k_shard_ids(ShardArgs a) {
     __shared__ uint32_t tab[256];

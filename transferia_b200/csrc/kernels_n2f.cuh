@@ -45,6 +45,7 @@ __device__ __forceinline__ bool n2f_applies(const N2fArgs& a, const DCol& c, uin
     return !(c.aux && c.aux[r] == 1);
 }
 
+__global__ void k_n2f_sizes(N2fArgs a);
 #ifdef TF_KERNELS_N2F
 __global__ void __launch_bounds__(128) k_n2f_sizes(N2fArgs a) {
     const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -56,6 +57,7 @@ __global__ void __launch_bounds__(128) k_n2f_sizes(N2fArgs a) {
     a.out_len[(size_t)blockIdx.y * a.nrows + r] = out;
 }
 #endif  // TF_KERNELS_N2F
+__global__ void k_n2f_write(N2fArgs a);
 #ifdef TF_KERNELS_N2F
 __global__ void __launch_bounds__(128) k_n2f_write(N2fArgs a) {
     const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;

@@ -17,6 +17,7 @@ __device__ __forceinline__ uint32_t str_len(const DCol& c, const uint32_t* sel, 
 
 // encoded size (LEB128 length + payload) of every tile of TF_STR_TILE kept rows, for every String column
 #define TF_STR_GROUP 4      /* tiles per CTA: their loads are issued together, which hides the gather latency */
+__global__ void k_str_sizes(EncodeArgs a);
 #ifdef TF_KERNELS_STR
 __global__ void __launch_bounds__(TF_STR_THREADS) k_str_sizes(EncodeArgs a) {
     __shared__ uint32_t sm[33];
@@ -48,6 +49,7 @@ __device__ __forceinline__ uint32_t str_find_row(const uint32_t* ex, uint32_t x)
     for (int it = 0; it < 8; it++) { const uint32_t mid = (lo + hi) >> 1; if (ex[mid] <= x) lo = mid; else hi = mid; }
     return lo;
 }
+__global__ void k_encode_str_plain(EncodeArgs a);
 #ifdef TF_KERNELS_STR
 __global__ void __launch_bounds__(TF_STR_THREADS) k_encode_str_plain(EncodeArgs a) {
     __shared__ uint32_t sm[33];
@@ -125,6 +127,7 @@ __global__ void __launch_bounds__(TF_STR_THREADS) k_encode_str_plain(EncodeArgs 
 #endif  // TF_KERNELS_STR
 
 // LEB128 length + text of convert_to_string columns, one kept row per thread, staged in shared memory.
+__global__ void k_encode_str(EncodeArgs a);
 #ifdef TF_KERNELS_STR
 __global__ void __launch_bounds__(TF_STR_THREADS) k_encode_str(EncodeArgs a) {
     __shared__ uint32_t sm[33];

@@ -1,5 +1,6 @@
-// Host-callable launchers: every kernel family is compiled in its own translation unit (tu_*.cu) so that the
-// families build in parallel; tfgpu.cu sees the argument structs but none of the kernel bodies.
+// The one launcher of tfgpu.cu. Every kernel is declared in its family header (kernels_*.cuh) and defined there under the family's
+// TF_KERNELS_* guard, which only that family's translation unit (tu_*.cu) sets: the families compile in parallel, and tfgpu.cu,
+// which sees the declarations but none of the kernel bodies, launches them through the host stubs those units export.
 #pragma once
 #include <cuda_runtime.h>
 #include "kernels_encode.cuh"
@@ -13,48 +14,26 @@
 #include "kernels_json_out.cuh"
 #include "kernels_deflate.cuh"
 namespace tfk {
-void launch_k_strictify(dim3 grid, dim3 block, size_t smem, cudaStream_t s, StrictArgs a);
-void launch_k_filter(dim3 grid, dim3 block, size_t smem, cudaStream_t s, FilterArgs a);
-void launch_k_scan_blockcnt(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint32_t* blockcnt, uint32_t* blockoff, uint32_t nblocks, DState* st);
-void launch_k_collect_errors(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint8_t* errcode, const uint16_t* errstep, uint64_t nrows, DevRowErr* out, unsigned long long* counter, unsigned long long cap);
-void launch_k_compact_sel(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint8_t* keep, const uint32_t* blockoff, uint64_t nrows, uint32_t* sel);
-void launch_k_layout_scan(dim3 grid, dim3 block, size_t smem, cudaStream_t s, LayoutArgs a);
-void launch_k_layout_finish(dim3 grid, dim3 block, size_t smem, cudaStream_t s, LayoutArgs a);
-void launch_k_layout_columnar(dim3 grid, dim3 block, size_t smem, cudaStream_t s, LayoutArgs a, ColRegions* regions);
-void launch_k_encode_fixed(dim3 grid, dim3 block, size_t smem, cudaStream_t s, EncodeArgs a);
-void launch_k_pack_validity(dim3 grid, dim3 block, size_t smem, cudaStream_t s, EncodeArgs a);
-void launch_k_measure(dim3 grid, dim3 block, size_t smem, cudaStream_t s, MeasureArgs a);
-void launch_k_str_sizes(dim3 grid, dim3 block, size_t smem, cudaStream_t s, EncodeArgs a);
-void launch_k_encode_str_plain(dim3 grid, dim3 block, size_t smem, cudaStream_t s, EncodeArgs a);
-void launch_k_encode_str(dim3 grid, dim3 block, size_t smem, cudaStream_t s, EncodeArgs a);
-void launch_k_mask_encode(dim3 grid, dim3 block, size_t smem, cudaStream_t s, MaskArgs a);
-void launch_k_shard_ids(dim3 grid, dim3 block, size_t smem, cudaStream_t s, ShardArgs a);
-void launch_k_lz4_frames(dim3 grid, dim3 block, size_t smem, cudaStream_t s, Lz4Args a);
-void launch_k_frame_seal(dim3 grid, dim3 block, size_t smem, cudaStream_t s, FrameArgs a);
-void launch_k_csv_count_nl(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint8_t* text, uint64_t len, uint32_t* blk_cnt, const uint32_t* endbits);
-void launch_k_csv_line_index(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint8_t* text, uint64_t len, const uint32_t* blk_off, uint32_t* line_end, const uint32_t* endbits);
-void launch_k_widen_lens(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const LensSrc* src, uint64_t nrows, uint32_t* out);
-void launch_k_csv_pass1(dim3 grid, dim3 block, size_t smem, cudaStream_t s, CsvArgs a);
-void launch_k_csv_offsets(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint32_t* span_len, uint64_t nrows, uint32_t* offsets , uint64_t* col_total);
-void launch_k_offsets_sum(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint32_t* span_len, uint64_t nrows, uint32_t nchunks, uint64_t* chunk_sum);
-void launch_k_offsets_chunks(dim3 grid, dim3 block, size_t smem, cudaStream_t s, uint64_t* chunk_sum, uint32_t nchunks, uint64_t* col_total);
-void launch_k_offsets_write(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint32_t* span_len, uint64_t nrows, uint32_t nchunks, const uint64_t* chunk_base, const uint64_t* col_total, uint32_t* offsets);
-void launch_k_csv_pass2(dim3 grid, dim3 block, size_t smem, cudaStream_t s, CsvCopyArgs a);
-void launch_k_json_mark_msgs(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint64_t* msg_end, uint32_t nmsgs, uint32_t* bits);
-void launch_k_json_count_nonempty(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint8_t* text, const uint32_t* line_end, uint64_t nlines, uint32_t* blk_cnt);
-void launch_k_json_rank(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint8_t* text, const uint32_t* line_end, uint64_t nlines, const uint32_t* blk_off, uint32_t* rank);
-void launch_k_json_msg_first(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint64_t* msg_end, uint32_t nmsgs, const uint32_t* line_end, uint64_t nlines, const uint32_t* rank, uint32_t* msg_rank0);
-void launch_k_json_pass1(dim3 grid, dim3 block, size_t smem, cudaStream_t s, JsnArgs a);
-void launch_k_json_pass2(dim3 grid, dim3 block, size_t smem, cudaStream_t s, JsnWriteArgs w);
-void launch_k_n2f_sizes(dim3 grid, dim3 block, size_t smem, cudaStream_t s, N2fArgs a);
-void launch_k_n2f_write(dim3 grid, dim3 block, size_t smem, cudaStream_t s, N2fArgs a);
-void launch_k_dbz_pass1(dim3 grid, dim3 block, size_t smem, cudaStream_t s, DbzArgs a);
-void launch_k_dbz_pass2(dim3 grid, dim3 block, size_t smem, cudaStream_t s, DbzWriteArgs w);
-void launch_k_json_sizes(dim3 grid, dim3 block, size_t smem, cudaStream_t s, JsonArgs a);
-void launch_k_json_write(dim3 grid, dim3 block, size_t smem, cudaStream_t s, JsonArgs a);
-cudaError_t dbz_kernels_init();   // dynamic shared memory limit of k_dbz_pass1
-void launch_k_deflate_chunks(dim3 grid, dim3 block, size_t smem, cudaStream_t s, DeflateArgs a);
-void launch_k_deflate_finish(dim3 grid, dim3 block, size_t smem, cudaStream_t s, DeflateArgs a);
-cudaError_t deflate_kernels_init();   // dynamic shared memory limit of k_deflate_chunks
-cudaError_t lz4_kernels_init();   // dynamic shared memory limits of k_lz4_frames / k_frame_seal
+struct CudaError { cudaError_t e; const char* what; };      // a failed CUDA call; `what` names the call, or the kernel of a launch
+
+// Launches kernel k on stream s and counts the launch in e->launches. With profiling on, a pair of CUDA events named after the
+// kernel brackets it; the first launch of a new entry-point call (e->call, stamped by on_device) starts the profile afresh, so the
+// profile holds every launch of the last call that launched anything. A launch the runtime refuses throws CudaError naming the kernel.
+template <typename E, typename... P, typename... A>
+void launch_kernel(E* e, const char* name, void (*k)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, const A&... args) {
+    e->launches++;
+    if (e->prof_on) {
+        if (e->prof_call != e->call) { e->prof_call = e->call; e->prof_n = 0; }
+        while ((int)e->prof_ev.size() < 2 * (e->prof_n + 1)) { cudaEvent_t ev; cudaEventCreate(&ev); e->prof_ev.push_back(ev); }
+        if ((int)e->prof_names.size() <= e->prof_n) e->prof_names.resize(e->prof_n + 1);
+        e->prof_names[e->prof_n] = name; cudaEventRecord(e->prof_ev[2 * e->prof_n], s);
+    }
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s;
+    const cudaError_t r = cudaLaunchKernelEx(&cfg, k, args...);
+    if (e->prof_on) { cudaEventRecord(e->prof_ev[2 * e->prof_n + 1], s); e->prof_n++; }
+    if (r != cudaSuccess) throw CudaError{r, name};
+}
 }  // namespace tfk
+// TF_LAUNCH(e, k_x, grid, block, smem, stream, args...): the profile name is the kernel's own
+#define TF_LAUNCH(e, k, ...) ::tfk::launch_kernel(e, #k, k, __VA_ARGS__)

@@ -22,7 +22,6 @@ using namespace tfk;
 
 namespace {
 
-struct CudaError { cudaError_t e; const char* what; };
 #define CK(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) throw CudaError{_e, #x}; } while (0)
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -104,17 +103,11 @@ struct tfgpu_engine {
     DbzEmitArgs dbz{};                                 // set by tfgpu_emit_debezium for the TF_WIRE_DEBEZIUM branch of run_chain
     unsigned long long* lz_phases = nullptr;      // debug: per-phase cycle counters of k_lz4_frames
     void* work_json_sizes(uint64_t n) { json_sizes.ensure(n * 4 + 256); return json_sizes.p; }
-    // optional per-kernel CUDA-event timing of the last call (bench roofline)
+    // optional per-kernel CUDA-event timing of the last call that launched anything (bench roofline), kept by launch_kernel:
+    // `call` numbers the entry-point calls, `prof_call` is the one the profile holds
+    uint64_t call = 0, prof_call = 0;
     bool prof_on = false; std::vector<cudaEvent_t> prof_ev; std::vector<const char*> prof_names; int prof_n = 0;
     std::string prof_json;
-    void prof_begin(const char* name, cudaStream_t s) {
-        launches++;
-        if (!prof_on) return;
-        while ((int)prof_ev.size() < 2 * (prof_n + 1)) { cudaEvent_t ev; cudaEventCreate(&ev); prof_ev.push_back(ev); }
-        if ((int)prof_names.size() <= prof_n) prof_names.resize(prof_n + 1);
-        prof_names[prof_n] = name; cudaEventRecord(prof_ev[2 * prof_n], s);
-    }
-    void prof_end(cudaStream_t s) { if (!prof_on) return; cudaEventRecord(prof_ev[2 * prof_n + 1], s); prof_n++; }
 };
 
 struct tfgpu_result {
@@ -148,6 +141,7 @@ int cuda_fail(tfgpu_engine* e, const CudaError& c) {
 // The exception boundary of every entry point that takes an engine: selects its device, runs `body` (which returns a TF_* code)
 // and turns what it throws into a code, with the message in e->last_error. Nothing crosses extern "C".
 template <typename F> int on_device(tfgpu_engine* e, F&& body) {
+    e->call++;
     try {
         CK(cudaSetDevice(e->device));
         return body();
@@ -307,12 +301,12 @@ Sizes compute_sizes(const tfgpu_engine* e, const PlanDev& pd, const tf_batch* in
 // exclusive scan of the text-cell lengths of every var-width column: offsets[slot][row], col_total[slot]
 static void launch_offsets(tfgpu_engine* e, const uint32_t* d_len, uint64_t nrows, uint32_t nslots, uint32_t* d_off, uint64_t* d_tot, cudaStream_t s) {
     const uint32_t nchunks = (uint32_t)((nrows + CSV_OFF_CHUNK - 1) / CSV_OFF_CHUNK);
-    if (!nchunks || !nslots) { launch_k_csv_offsets(nslots ? nslots : 1, 1024, 0, s, d_len, nrows, d_off, d_tot); return; }
+    if (!nchunks || !nslots) { TF_LAUNCH(e, k_csv_offsets, nslots ? nslots : 1, 1024, 0, s, d_len, nrows, d_off, d_tot); return; }
     e->off_scratch.ensure((size_t)nslots * nchunks * 8 + 256);
     uint64_t* cs = (uint64_t*)e->off_scratch.p;
-    e->prof_begin("k_offsets_sum", s); launch_k_offsets_sum(dim3(nchunks, nslots), 1024, 0, s, d_len, nrows, nchunks, cs); e->prof_end(s);
-    e->prof_begin("k_offsets_chunks", s); launch_k_offsets_chunks(nslots, 32, 0, s, cs, nchunks, d_tot); e->prof_end(s);
-    e->prof_begin("k_offsets_write", s); launch_k_offsets_write(dim3(nchunks, nslots), 1024, 0, s, d_len, nrows, nchunks, cs, d_tot, d_off); e->prof_end(s);
+    TF_LAUNCH(e, k_offsets_sum, dim3(nchunks, nslots), 1024, 0, s, d_len, nrows, nchunks, cs);
+    TF_LAUNCH(e, k_offsets_chunks, nslots, 32, 0, s, cs, nchunks, d_tot);
+    TF_LAUNCH(e, k_offsets_write, dim3(nchunks, nslots), 1024, 0, s, d_len, nrows, nchunks, cs, d_tot, d_off);
 }
 
 // Text heaps of k var-width columns whose cell lengths are d_len [k][nrows]: offsets d_off [k][nrows+1] and totals d_tot [k] on the
@@ -370,9 +364,9 @@ void run_deflate(tfgpu_engine* e, const uint8_t* text, uint64_t total, bool zlib
     DeflateArgs da{text, total, e->wire.p, (unsigned long long*)(M + o_pfx), (uint32_t*)(M + o_sums), (uint32_t*)(M + o_ticket), (uint32_t)nch, zlib ? 1 : 0, e->d_state};
     if (nch) {
         const uint32_t grid = (uint32_t)std::min<uint64_t>(nch, (uint64_t)e->sm_count * 2);     // two CTAs of ~105 KiB per SM
-        e->prof_begin("k_deflate_chunks", s); launch_k_deflate_chunks(grid, DF_THREADS, df_smem().total, s, da); e->prof_end(s);
+        TF_LAUNCH(e, k_deflate_chunks, grid, DF_THREADS, df_smem().total, s, da);
     }
-    e->prof_begin("k_deflate_finish", s); launch_k_deflate_finish(1, 1024, 0, s, da); e->prof_end(s);
+    TF_LAUNCH(e, k_deflate_finish, 1, 1024, 0, s, da);
 }
 
 void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* dev_cols, const uint8_t* dev_kinds, int wire_fmt, const uint8_t* pre_err = nullptr) {
@@ -427,7 +421,6 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
             if (!d.in_w && !d.offsets) throw tfplan::FatalError(TF_E_FATAL_ARG, "column " + std::to_string(c) + ": offsets pointer is NULL");
         }
     }
-    if (!pre_err) e->prof_n = 0;
     const uint16_t* pre_term = nullptr;
     if (!strict.empty() && n) {        // Strictify pre-pass: loose fixed-width values -> the schema's type, range / cast failures as row errors
         Layout S;
@@ -440,7 +433,7 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
         CK(cudaMemcpyAsync(B + o_desc, strict.data(), strict.size() * sizeof(StrictCol), cudaMemcpyHostToDevice, s));
         if (pre_err) CK(cudaMemcpyAsync(B + o_err, pre_err, n, cudaMemcpyDeviceToDevice, s)); else CK(cudaMemsetAsync(B + o_err, 0, n, s));
         StrictArgs sa{(const StrictCol*)(B + o_desc), (int)strict.size(), n, B + o_err, (uint16_t*)(B + o_term)};
-        e->prof_begin("k_strictify", s); launch_k_strictify((uint32_t)((n + 255) / 256), 256, 0, s, sa); e->prof_end(s);
+        TF_LAUNCH(e, k_strictify, (uint32_t)((n + 255) / 256), 256, 0, s, sa);
         pre_err = B + o_err; pre_term = (const uint16_t*)(B + o_term);
     }
     CK(cudaMemcpyAsync(e->d_cols, hc.data(), sizeof(DCol) * nc, cudaMemcpyHostToDevice, s));
@@ -455,11 +448,11 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
         CK(cudaMemcpyAsync(B + o_which, which.data(), k2 * 4, cudaMemcpyHostToDevice, s));
         if (pre_err) CK(cudaMemcpyAsync(B + o_err, pre_err, n, cudaMemcpyDeviceToDevice, s)); else CK(cudaMemsetAsync(B + o_err, 0, n, s));
         N2fArgs na{e->d_cols, (const int32_t*)(B + o_which), dev_kinds, n, (uint32_t*)(B + o_len), (const uint32_t*)(B + o_off), nullptr, (const uint64_t*)(B + o_base), B + o_err};
-        e->prof_begin("k_n2f_sizes", s); launch_k_n2f_sizes(dim3((uint32_t)((n + 127) / 128), (uint32_t)k2), 128, 0, s, na); e->prof_end(s);
+        TF_LAUNCH(e, k_n2f_sizes, dim3((uint32_t)((n + 127) / 128), (uint32_t)k2), 128, 0, s, na);
         const Heaps h = size_heaps(e, (const uint32_t*)(B + o_len), n, (uint32_t)k2, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), (uint64_t*)(B + o_base),
                                    e->n2f_heap, "number_to_float: a rewritten column exceeds 4 GiB");
         na.heap = e->n2f_heap.p;
-        e->prof_begin("k_n2f_write", s); launch_k_n2f_write(dim3((uint32_t)((n + 127) / 128), (uint32_t)k2), 128, 0, s, na); e->prof_end(s);
+        TF_LAUNCH(e, k_n2f_write, dim3((uint32_t)((n + 127) / 128), (uint32_t)k2), 128, 0, s, na);
         for (size_t k = 0; k < k2; k++) { DCol& d = hc[pl.n2f_cols[k]]; d.offsets = (const uint32_t*)(B + o_off) + k * (n + 1); d.heap = e->n2f_heap.p + h.base[k]; }
         CK(cudaMemcpyAsync(e->d_cols, hc.data(), sizeof(DCol) * nc, cudaMemcpyHostToDevice, s));
         pre_err = B + o_err;                 // parser errors carried over + N2F_HOST rows
@@ -472,9 +465,9 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
     const uint32_t nb = (uint32_t)((n + 255) / 256);
     if (has_filter && n) {
         FilterArgs fa{e->d_cols, dev_kinds, n, pd.d_fsteps, pd.n_fsteps, pd.d_expr_off, pd.d_terms, pd.d_blob, e->keep, e->errcode, e->errstep, e->blockcnt, e->d_state, pre_err, pre_term, sink_guard ? 1 : 0};
-        e->prof_begin("k_filter", s); launch_k_filter(nb, 256, 0, s, fa); e->prof_end(s);
-        e->prof_begin("k_scan_blockcnt", s); launch_k_scan_blockcnt(1, 1024, 0, s, e->blockcnt, e->blockoff, nb, e->d_state); e->prof_end(s);
-        e->prof_begin("k_compact_sel", s); launch_k_compact_sel(nb, 256, 0, s, e->keep, e->blockoff, n, e->sel); e->prof_end(s);
+        TF_LAUNCH(e, k_filter, nb, 256, 0, s, fa);
+        TF_LAUNCH(e, k_scan_blockcnt, 1, 1024, 0, s, e->blockcnt, e->blockoff, nb, e->d_state);
+        TF_LAUNCH(e, k_compact_sel, nb, 256, 0, s, e->keep, e->blockoff, n, e->sel);
     }
     const uint32_t* sel = (has_filter && n) ? e->sel : nullptr;
     const uint32_t ntiles = (uint32_t)((n + TF_STR_TILE - 1) / TF_STR_TILE);
@@ -490,7 +483,7 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
     if (pl.has_sharder && n) {
         e->part_ids.ensure(n * 4 + 256);
         ShardArgs sa{e->d_cols, pd.d_shard_cols, (int)pl.shard_cols.size(), pd.d_mask_keys, sel, e->d_state, pl.shards, (uint32_t*)e->part_ids.p};
-        e->prof_begin("k_shard_ids", s); launch_k_shard_ids(nb, 256, 0, s, sa); e->prof_end(s);
+        TF_LAUNCH(e, k_shard_ids, nb, 256, 0, s, sa);
     }
     e->last_has_sharder = pl.has_sharder;
     if (json_rows) {
@@ -501,26 +494,25 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
                     dbz ? 3 : ser ? (wire_base == TF_WIRE_SER_JSON ? 1 : 2) : 0, (uint32_t)(((wire_fmt & TF_WIRE_F_CLOSING_NEWLINE) ? TF_SER_NL : 0) | ((wire_fmt & TF_WIRE_F_ANY_AS_STRING) ? TF_SER_AAS : 0)), e->errcode, e->errstep, DbzEmitArgs{}};
         if (dbz) { ja.jcols = pd.d_sjcols; e->dbz_keysz.ensure(n * 4 + 256); e->dbz_msgsz.ensure(n * 28 + 256); ja.dz = e->dbz; ja.dz.key_size = (uint32_t*)e->dbz_keysz.p; ja.dz.msg_size = (uint32_t*)e->dbz_msgsz.p; }
         if (ser && !has_filter && n) { CK(cudaMemsetAsync(e->errcode, 0, n, s)); CK(cudaMemsetAsync(e->errstep, 0, 2 * n, s)); }
-        if (jt) { e->prof_begin("k_json_sizes", s); launch_k_json_sizes(jt, TF_JSON_TILE, 0, s, ja); e->prof_end(s); }
+        if (jt) TF_LAUNCH(e, k_json_sizes, jt, TF_JSON_TILE, 0, s, ja);
         LayoutArgs lj{e->d_cols, 0, pd.d_out_cols, pd.d_str_slots, 1, e->tile_sum, e->tile_base, sz.ntiles_cap, pd.d_col_headers, pd.d_col_header_off,
                       e->raw.p, e->d_state, n, 1, e->frame_bytes, e->col_bytes};
-        e->prof_begin("k_layout_scan", s); launch_k_layout_scan(1, 1024, 0, s, lj); e->prof_end(s);
+        TF_LAUNCH(e, k_layout_scan, 1, 1024, 0, s, lj);
         uint64_t json_total = 0;
         {   // row text has no useful upper bound ('f' floats reach 300+ characters): size the output from the measured total
             CK(cudaMemcpyAsync(&json_total, e->col_bytes, 8, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
             e->raw.ensure(json_total + 256); ja.raw = e->raw.p;
         }
-        e->prof_begin("k_json_write", s); launch_k_json_write(jt ? jt : 1, TF_JSON_TILE, 0, s, ja); e->prof_end(s);
+        TF_LAUNCH(e, k_json_write, jt ? jt : 1, TF_JSON_TILE, 0, s, ja);
         if (ser && (wire_fmt & (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB))) run_deflate(e, e->raw.p, n ? json_total : 0, (wire_fmt & TF_WIRE_F_ZLIB) != 0);
-        CK(cudaGetLastError());
         return;
     }
-    if (pd.n_str && ntiles) { e->prof_begin("k_str_sizes", s); launch_k_str_sizes(dim3(str_gx, pd.n_str), TF_STR_THREADS, 0, s, ea); e->prof_end(s); }
+    if (pd.n_str && ntiles) TF_LAUNCH(e, k_str_sizes, dim3(str_gx, pd.n_str), TF_STR_THREADS, 0, s, ea);
     LayoutArgs la{e->d_cols, (int)pl.out_cols.size(), pd.d_out_cols, pd.d_str_slots, pd.n_str, e->tile_sum, e->tile_base, sz.ntiles_cap, pd.d_col_headers, pd.d_col_header_off,
                   e->raw.p, e->d_state, n, 1, e->frame_bytes, e->col_bytes};
-    if (pd.n_str) { e->prof_begin("k_layout_scan", s); launch_k_layout_scan(pd.n_str, 1024, 0, s, la); e->prof_end(s); }
+    if (pd.n_str) TF_LAUNCH(e, k_layout_scan, pd.n_str, 1024, 0, s, la);
     if (!columnar) {
-        e->prof_begin("k_layout_finish", s); launch_k_layout_finish(1, 256, 0, s, la); e->prof_end(s);
+        TF_LAUNCH(e, k_layout_finish, 1, 256, 0, s, la);
         if (n) {
             // (the fixed-width streams and the String columns write disjoint parts of the block, but running them on two streams
             // was measured slower than running them in sequence: both are latency-bound gathers that already fill the SMs)
@@ -528,13 +520,13 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
                 // widest stream is 8 bytes per row: words = 2n (+1 for misalignment)
                 const uint32_t gx = grid_cap(e, (uint32_t)((2 * n + 2 + TF_FIX_TILE_WORDS - 1) / TF_FIX_TILE_WORDS), (uint32_t)pd.n_fixed_slots, 6);
                 EncodeArgs fa = ea; fa.slots = pd.d_fixed_slots;
-                e->prof_begin("k_encode_fixed", s); launch_k_encode_fixed(dim3(gx, pd.n_fixed_slots), 256, 0, s, fa); e->prof_end(s);
+                TF_LAUNCH(e, k_encode_fixed, dim3(gx, pd.n_fixed_slots), 256, 0, s, fa);
             }
-            if (pd.n_str) { e->prof_begin("k_encode_str_plain", s); launch_k_encode_str_plain(dim3(str_gx, pd.n_str), TF_STR_THREADS, 0, s, ea); e->prof_end(s); }
-            if (pd.n_str && pd.n_tostr) { e->prof_begin("k_encode_str", s); launch_k_encode_str(dim3(ntiles, pd.n_str), TF_STR_THREADS, 0, s, ea); e->prof_end(s); }
+            if (pd.n_str) TF_LAUNCH(e, k_encode_str_plain, dim3(str_gx, pd.n_str), TF_STR_THREADS, 0, s, ea);
+            if (pd.n_str && pd.n_tostr) TF_LAUNCH(e, k_encode_str, dim3(ntiles, pd.n_str), TF_STR_THREADS, 0, s, ea);
             if (pd.n_mask_cols) {
                 MaskArgs ma{e->d_cols, pd.d_mask_slots, pd.d_mask_keys, sel, e->d_state, e->raw.p, 0};
-                e->prof_begin("k_mask_encode", s); launch_k_mask_encode(dim3((uint32_t)((n + 127) / 128), pd.n_mask_cols), 128, 0, s, ma); e->prof_end(s);
+                TF_LAUNCH(e, k_mask_encode, dim3((uint32_t)((n + 127) / 128), pd.n_mask_cols), 128, 0, s, ma);
             }
         }
     } else {
@@ -554,22 +546,22 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
         }
         std::vector<int32_t> both(fixed); both.insert(both.end(), valid.begin(), valid.end());
         if (!both.empty()) CK(cudaMemcpyAsync(e->d_call_slots, both.data(), both.size() * 4, cudaMemcpyHostToDevice, s));
-        e->prof_begin("k_layout_columnar", s); launch_k_layout_columnar(1, 256, 0, s, la, e->d_regions); e->prof_end(s);
+        TF_LAUNCH(e, k_layout_columnar, 1, 256, 0, s, la, e->d_regions);
         if (n) {
             if (!fixed.empty()) {
                 const uint32_t gx = grid_cap(e, (uint32_t)((2 * n + 2 + TF_FIX_TILE_WORDS - 1) / TF_FIX_TILE_WORDS), (uint32_t)fixed.size(), 6);
                 EncodeArgs fa = ea; fa.slots = e->d_call_slots;
-                e->prof_begin("k_encode_fixed", s); launch_k_encode_fixed(dim3(gx, (uint32_t)fixed.size()), 256, 0, s, fa); e->prof_end(s);
+                TF_LAUNCH(e, k_encode_fixed, dim3(gx, (uint32_t)fixed.size()), 256, 0, s, fa);
             }
             if (!valid.empty()) {
                 EncodeArgs va = ea; va.slots = e->d_call_slots + fixed.size();
-                e->prof_begin("k_pack_validity", s); launch_k_pack_validity(dim3((uint32_t)((n / 8 + 256) / 256), (uint32_t)valid.size()), 256, 0, s, va); e->prof_end(s);
+                TF_LAUNCH(e, k_pack_validity, dim3((uint32_t)((n / 8 + 256) / 256), (uint32_t)valid.size()), 256, 0, s, va);
             }
-            if (pd.n_str) { e->prof_begin("k_encode_str_plain", s); launch_k_encode_str_plain(dim3(str_gx, pd.n_str), TF_STR_THREADS, 0, s, ea); e->prof_end(s); }
-            if (pd.n_str && pd.n_tostr) { e->prof_begin("k_encode_str", s); launch_k_encode_str(dim3(ntiles, pd.n_str), TF_STR_THREADS, 0, s, ea); e->prof_end(s); }
+            if (pd.n_str) TF_LAUNCH(e, k_encode_str_plain, dim3(str_gx, pd.n_str), TF_STR_THREADS, 0, s, ea);
+            if (pd.n_str && pd.n_tostr) TF_LAUNCH(e, k_encode_str, dim3(ntiles, pd.n_str), TF_STR_THREADS, 0, s, ea);
             if (pd.n_mask_cols) {
                 MaskArgs ma{e->d_cols, pd.d_mask_slots, pd.d_mask_keys, sel, e->d_state, e->raw.p, 1};
-                e->prof_begin("k_mask_encode", s); launch_k_mask_encode(dim3((uint32_t)((n + 127) / 128), pd.n_mask_cols), 128, 0, s, ma); e->prof_end(s);
+                TF_LAUNCH(e, k_mask_encode, dim3((uint32_t)((n + 127) / 128), pd.n_mask_cols), 128, 0, s, ma);
             }
         }
     }
@@ -581,16 +573,15 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
         join_tail(e);            // the previous batch's checksum kernel still reads the wire bytes and sizes this kernel overwrites
         CK(cudaMemsetAsync(e->frame_pfx, 0, sz.n_frames_max * 8, s));
         // frames are compressed and written at their final wire offset by one kernel (sizes of the earlier frames by decoupled look-back)
-        e->prof_begin("k_lz4_frames", s); launch_k_lz4_frames(grid, LZ_THREADS, smem, s, za); e->prof_end(s);
+        TF_LAUNCH(e, k_lz4_frames, grid, LZ_THREADS, smem, s, za);
         // the checksum kernel (one thread per frame: latency-bound, a few warps per SM) runs on the side stream, under the next batch
         FrameArgs fa{e->comp_size, e->wire_off, e->wire.p, e->d_tail};
         cudaStream_t s3 = e->side_stream;
         CK(cudaEventRecord(e->ev_fork, s)); CK(cudaStreamWaitEvent(s3, e->ev_fork, 0));
-        e->prof_begin("k_frame_seal", s3); launch_k_frame_seal((uint32_t)((sz.n_frames_max + 31) / 32), 32, SEAL_SMEM, s3, fa); e->prof_end(s3);
+        TF_LAUNCH(e, k_frame_seal, (uint32_t)((sz.n_frames_max + 31) / 32), 32, SEAL_SMEM, s3, fa);
         CK(cudaEventRecord(e->ev_tail, s3));
         e->tail_pending = true; e->tail_nrows = n; e->tail_plan = (const void*)&pd; e->tail_nframes_max = sz.n_frames_max;      // joined by whoever needs the wire bytes, or by the next batch before its LZ4
     }
-    CK(cudaGetLastError());
 }
 
 }  // namespace
@@ -634,7 +625,11 @@ int tfgpu_engine_create(const char* cfg_json, const int* device_ids, int n_devic
         CK(cudaMalloc(&e->d_tail, 64)); CK(cudaMemset(e->d_tail, 0, 64));
         CK(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
         CK(cudaMalloc(&e->d_state, sizeof(DState)));
-        CK(lz4_kernels_init()); CK(dbz_kernels_init()); CK(deflate_kernels_init());
+        // kernels whose dynamic shared memory passes the 48 KiB default
+        const struct { const void* k; size_t smem; } big_smem[] = {
+            {(const void*)k_lz4_frames, lz_smem(LZ_MAX_FRAME).total}, {(const void*)k_frame_seal, SEAL_SMEM},
+            {(const void*)k_dbz_pass1, DBZ_STAGE}, {(const void*)k_deflate_chunks, df_smem().total}};
+        for (const auto& b : big_smem) CK(cudaFuncSetAttribute(b.k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b.smem));
     } catch (const CudaError& c) { return c.e == cudaErrorMemoryAllocation ? TF_E_RETRY_OOM : TF_E_RETRY_LAUNCH; }
     catch (const std::exception&) { return TF_E_FATAL_CONFIG; }
     *out = e.release();
@@ -802,8 +797,7 @@ int tfgpu_push_encode_selective(tfgpu_engine* e, int plan_id, int wire_fmt, cons
         e->sel_stage.ensure(L.total() + 256);
         uint8_t* B = e->sel_stage.p + o_flags;
         FilterArgs fa{e->d_cols, dev_kinds, n, pd.d_fsteps, pd.n_fsteps, pd.d_expr_off, pd.d_terms, pd.d_blob, B, B + n, (uint16_t*)(B + 2 * n), (uint32_t*)(e->sel_stage.p + o_blockcnt), e->d_state, nullptr, nullptr, 0};
-        e->prof_n = 0;
-        e->prof_begin("k_filter", s); launch_k_filter(nb, 256, 0, s, fa); e->prof_end(s);
+        TF_LAUNCH(e, k_filter, nb, 256, 0, s, fa);
         if (e->sel_host_cap < 4 * n) { if (e->sel_host) CK(cudaFreeHost(e->sel_host)); e->sel_host = nullptr; e->sel_host_cap = 0; const size_t want = align_up(4 * n + n + 4096, 1 << 16); CK(cudaMallocHost(&e->sel_host, want)); e->sel_host_cap = want; }
         CK(cudaMemcpyAsync(e->sel_host, B, 4 * n, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
@@ -852,7 +846,7 @@ static void expand_lens(tfgpu_engine* e, uint64_t nr, std::vector<tf_col>& dv, D
     uint8_t* B = larena.p; cudaStream_t st = e->stream;
     CK(cudaMemcpyAsync(B + o_src, src.data(), K * sizeof(LensSrc), cudaMemcpyHostToDevice, st));
     // `src` is pageable: cudaMemcpyAsync has staged it before it returns, so the vector may go out of scope and nothing waits here
-    if (nr) { e->launches++; launch_k_widen_lens(dim3((uint32_t)std::min<uint64_t>((nr + 255) / 256, 2048), (uint32_t)K), 256, 0, st, (const LensSrc*)(B + o_src), nr, (uint32_t*)(B + o_len)); }
+    if (nr) TF_LAUNCH(e, k_widen_lens, dim3((uint32_t)std::min<uint64_t>((nr + 255) / 256, 2048), (uint32_t)K), 256, 0, st, (const LensSrc*)(B + o_src), nr, (uint32_t*)(B + o_len));
     launch_offsets(e, (const uint32_t*)(B + o_len), nr, (uint32_t)K, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), st);
     for (size_t k = 0; k < K; k++) { dv[which[k]].offsets = (const uint32_t*)(B + o_off) + k * (nr + 1); dv[which[k]].flags &= ~(TF_COL_LENS8 | TF_COL_LENS16); }
 }
@@ -918,7 +912,7 @@ static void fetch_errors(tfgpu_engine* e, uint64_t n, tfgpu_result* r) {
         e->err_list.ensure(cap * sizeof(DevRowErr) + 64);
         unsigned long long* counter = (unsigned long long*)e->err_list.p; DevRowErr* list = (DevRowErr*)(e->err_list.p + 16);
         CK(cudaMemsetAsync(counter, 0, 8, s));
-        e->launches++; launch_k_collect_errors((uint32_t)((n + 255) / 256), 256, 0, s, e->errcode, e->errstep, n, list, counter, cap);
+        TF_LAUNCH(e, k_collect_errors, (uint32_t)((n + 255) / 256), 256, 0, s, e->errcode, e->errstep, n, list, counter, cap);
         got.resize(cap); unsigned long long found = 0;
         CK(cudaMemcpyAsync(got.data(), list, cap * sizeof(DevRowErr), cudaMemcpyDeviceToHost, s));
         CK(cudaMemcpyAsync(&found, counter, 8, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
@@ -1214,8 +1208,7 @@ int tfgpu_measure(tfgpu_engine* e, const tf_batch* in, uint64_t* per_row, uint64
         unsigned long long* d_total = (unsigned long long*)e->work.p; uint64_t* d_rows = per_row ? (uint64_t*)(e->work.p + 64) : nullptr;
         CK(cudaMemcpyAsync(e->d_cols, hc.data(), sizeof(DCol) * nc, cudaMemcpyHostToDevice, s));
         CK(cudaMemsetAsync(d_total, 0, 8, s));
-        e->prof_n = 0;
-        if (n) { MeasureArgs ma{e->d_cols, (int)nc, n, d_rows, d_total}; e->prof_begin("k_measure", s); launch_k_measure((uint32_t)((n + 255) / 256), 256, 0, s, ma); e->prof_end(s); CK(cudaGetLastError()); }
+        if (n) { MeasureArgs ma{e->d_cols, (int)nc, n, d_rows, d_total}; TF_LAUNCH(e, k_measure, (uint32_t)((n + 255) / 256), 256, 0, s, ma); }
         CK(cudaMemcpyAsync(total, d_total, 8, cudaMemcpyDeviceToHost, s));
         if (per_row && n) CK(cudaMemcpyAsync(per_row, d_rows, n * 8, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
@@ -1336,9 +1329,8 @@ int tfgpu_parse_csv(tfgpu_engine* e, int plan_id, const char* opts_json, const u
         uint32_t* blk_cnt = (uint32_t*)(e->work.p + w_cnt); uint32_t* blk_off = (uint32_t*)(e->work.p + w_off);
         if (nblk) {
             CK(cudaMemsetAsync(e->d_state, 0, sizeof(DState), s));
-            e->prof_n = 0;
-            e->prof_begin("k_csv_count_nl", s); launch_k_csv_count_nl(nblk, 256, 0, s, d_text, len, blk_cnt, nullptr); e->prof_end(s);
-            e->prof_begin("k_scan_blockcnt", s); launch_k_scan_blockcnt(1, 1024, 0, s, blk_cnt, blk_off, nblk, e->d_state); e->prof_end(s);
+            TF_LAUNCH(e, k_csv_count_nl, nblk, 256, 0, s, d_text, len, blk_cnt, nullptr);
+            TF_LAUNCH(e, k_scan_blockcnt, 1, 1024, 0, s, blk_cnt, blk_off, nblk, e->d_state);
             DState st; CK(cudaMemcpyAsync(&st, e->d_state, sizeof st, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
             nlines = st.n_kept;
         }
@@ -1380,18 +1372,18 @@ int tfgpu_parse_csv(tfgpu_engine* e, int plan_id, const char* opts_json, const u
         CK(cudaMemcpyAsync(B + o_ns, next_same.data(), nc * 2, cudaMemcpyHostToDevice, s));
         CK(cudaMemcpyAsync(B + o_blob, ho.blob.data(), ho.blob.size(), cudaMemcpyHostToDevice, s));
         Heaps h; const uint8_t* heap = nullptr;
-        if (nlines) { e->prof_begin("k_csv_line_index", s); launch_k_csv_line_index(nblk, 256, 0, s, d_text, len, blk_off, (uint32_t*)(B + o_line), nullptr); e->prof_end(s); }
+        if (nlines) TF_LAUNCH(e, k_csv_line_index, nblk, 256, 0, s, d_text, len, blk_off, (uint32_t*)(B + o_line), nullptr);
         if (nrows) {
             CsvArgs ca{d_text, len, (const uint32_t*)(B + o_line), nlines, skip, ho.cfg, B + o_blob, (const CsvColDev*)(B + o_cols), (int)nc,
                        (const int16_t*)(B + o_fc), nfields, (const int16_t*)(B + o_ns), (uint32_t*)(B + o_ss), (uint32_t*)(B + o_sl), (uint32_t*)(B + o_sr), B + o_err};
-            e->prof_begin("k_csv_pass1", s); launch_k_csv_pass1((uint32_t)std::min<uint64_t>((nrows + CSV_TILE_ROWS - 1) / CSV_TILE_ROWS, (uint64_t)e->sm_count * 16), 32 * CSV_WARPS, 0, s, ca); e->prof_end(s);
+            TF_LAUNCH(e, k_csv_pass1, (uint32_t)std::min<uint64_t>((nrows + CSV_TILE_ROWS - 1) / CSV_TILE_ROWS, (uint64_t)e->sm_count * 16), 32 * CSV_WARPS, 0, s, ca);
             if (nslots) {
                 // text heaps (the staged batch lives in csv_stage, in_arena is free)
                 h = size_heaps(e, (const uint32_t*)(B + o_sl), nrows, (uint32_t)nslots, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), (uint64_t*)(B + o_base),
                                e->in_arena, "csv chunk: a text column exceeds 4 GiB");
                 heap = e->in_arena.p;
                 CsvCopyArgs cp{d_text, (const uint32_t*)(B + o_ss), (const uint32_t*)(B + o_sl), (const uint32_t*)(B + o_sr), (const uint32_t*)(B + o_off), e->in_arena.p, (const uint64_t*)(B + o_base), nrows, ho.cfg.quote};
-                e->prof_begin("k_csv_pass2", s); launch_k_csv_pass2(dim3((uint32_t)((nrows + 255) / 256), nslots), 256, 0, s, cp); e->prof_end(s);
+                TF_LAUNCH(e, k_csv_pass2, dim3((uint32_t)((nrows + 255) / 256), nslots), 256, 0, s, cp);
             }
         }
         // the staged batch, device resident
@@ -1472,15 +1464,14 @@ int tfgpu_parse_json(tfgpu_engine* e, int plan_id, const char* opts_json, const 
             uint8_t* W = e->json_msgs.p;
             uint32_t* blk_cnt = (uint32_t*)(W + w_cnt); uint32_t* blk_off = (uint32_t*)(W + w_off); uint32_t* endbits = (uint32_t*)(W + w_bits);
             uint64_t nlines = 0;
-            e->prof_n = 0;
             if (nblk) {
                 CK(cudaMemsetAsync(e->d_state, 0, sizeof(DState), s));
                 CK(cudaMemsetAsync(endbits, 0, bits_words * 4, s));
                 CK(cudaMemcpyAsync(W + w_end, h_end.data(), (size_t)n_msgs * 8, cudaMemcpyHostToDevice, s)); CK(cudaMemcpyAsync(W + w_moff, h_off.data(), (size_t)n_msgs * 8, cudaMemcpyHostToDevice, s));
                 CK(cudaMemcpyAsync(W + w_ws, h_ws.data(), (size_t)n_msgs * 8, cudaMemcpyHostToDevice, s)); CK(cudaMemcpyAsync(W + w_wn, h_wn.data(), (size_t)n_msgs * 4, cudaMemcpyHostToDevice, s));
-                e->prof_begin("k_json_mark_msgs", s); launch_k_json_mark_msgs((n_msgs + 255) / 256, 256, 0, s, (const uint64_t*)(W + w_end), n_msgs, endbits); e->prof_end(s);
-                e->prof_begin("k_csv_count_nl", s); launch_k_csv_count_nl(nblk, 256, 0, s, d_text, len, blk_cnt, endbits); e->prof_end(s);
-                e->prof_begin("k_scan_blockcnt", s); launch_k_scan_blockcnt(1, 1024, 0, s, blk_cnt, blk_off, nblk, e->d_state); e->prof_end(s);
+                TF_LAUNCH(e, k_json_mark_msgs, (n_msgs + 255) / 256, 256, 0, s, (const uint64_t*)(W + w_end), n_msgs, endbits);
+                TF_LAUNCH(e, k_csv_count_nl, nblk, 256, 0, s, d_text, len, blk_cnt, endbits);
+                TF_LAUNCH(e, k_scan_blockcnt, 1, 1024, 0, s, blk_cnt, blk_off, nblk, e->d_state);
                 DState st; CK(cudaMemcpyAsync(&st, e->d_state, sizeof st, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
                 nlines = st.n_kept;
             }
@@ -1514,11 +1505,11 @@ int tfgpu_parse_json(tfgpu_engine* e, int plan_id, const char* opts_json, const 
                 CK(cudaMemcpyAsync(B + o_cols, hc.data(), nc * sizeof(JsnColDev), cudaMemcpyHostToDevice, s));
                 CK(cudaMemcpyAsync(B + o_names, names.data(), names.size(), cudaMemcpyHostToDevice, s));
                 CK(cudaMemsetAsync(B + o_sl, 0, (size_t)nf * nrows * 4, s));
-                e->prof_begin("k_csv_line_index", s); launch_k_csv_line_index(nblk, 256, 0, s, d_text, len, blk_off, (uint32_t*)(B + o_line), endbits); e->prof_end(s);
-                e->prof_begin("k_json_count_nonempty", s); launch_k_json_count_nonempty(nlb, 128, 0, s, d_text, (const uint32_t*)(B + o_line), nlines, (uint32_t*)(B + o_lcnt)); e->prof_end(s);
-                e->prof_begin("k_scan_blockcnt", s); launch_k_scan_blockcnt(1, 1024, 0, s, (const uint32_t*)(B + o_lcnt), (uint32_t*)(B + o_loff), nlb, e->d_state); e->prof_end(s);
-                e->prof_begin("k_json_rank", s); launch_k_json_rank(nlb, 128, 0, s, d_text, (const uint32_t*)(B + o_line), nlines, (const uint32_t*)(B + o_loff), (uint32_t*)(B + o_rank)); e->prof_end(s);
-                e->prof_begin("k_json_msg_first", s); launch_k_json_msg_first((n_msgs + 255) / 256, 256, 0, s, (const uint64_t*)(W + w_end), n_msgs, (const uint32_t*)(B + o_line), nlines, (const uint32_t*)(B + o_rank), (uint32_t*)(W + w_r0)); e->prof_end(s);
+                TF_LAUNCH(e, k_csv_line_index, nblk, 256, 0, s, d_text, len, blk_off, (uint32_t*)(B + o_line), endbits);
+                TF_LAUNCH(e, k_json_count_nonempty, nlb, 128, 0, s, d_text, (const uint32_t*)(B + o_line), nlines, (uint32_t*)(B + o_lcnt));
+                TF_LAUNCH(e, k_scan_blockcnt, 1, 1024, 0, s, (const uint32_t*)(B + o_lcnt), (uint32_t*)(B + o_loff), nlb, e->d_state);
+                TF_LAUNCH(e, k_json_rank, nlb, 128, 0, s, d_text, (const uint32_t*)(B + o_line), nlines, (const uint32_t*)(B + o_loff), (uint32_t*)(B + o_rank));
+                TF_LAUNCH(e, k_json_msg_first, (n_msgs + 255) / 256, 256, 0, s, (const uint64_t*)(W + w_end), n_msgs, (const uint32_t*)(B + o_line), nlines, (const uint32_t*)(B + o_rank), (uint32_t*)(W + w_r0));
                 JsnArgs ja; std::memset(&ja, 0, sizeof ja);
                 ja.text = d_text; ja.len = len; ja.line_end = (const uint32_t*)(B + o_line); ja.nlines = nlines;
                 ja.msg_end = (const uint64_t*)(W + w_end); ja.msg_offset = (const uint64_t*)(W + w_moff); ja.msg_wsec = (const int64_t*)(W + w_ws); ja.msg_wnsec = (const uint32_t*)(W + w_wn); ja.nmsgs = n_msgs;
@@ -1528,7 +1519,7 @@ int tfgpu_parse_json(tfgpu_engine* e, int plan_id, const char* opts_json, const 
                 ja.part_off = part_off; ja.part_len = (uint32_t)partition.size();
                 ja.span_start = (uint32_t*)(B + o_ss); ja.span_len = (uint32_t*)(B + o_sl); ja.out_len = (uint32_t*)(B + o_len);
                 ja.err = B + o_err; ja.errcol = B + o_ecol;
-                e->prof_begin("k_json_pass1", s); launch_k_json_pass1(nlb, 128, JSN_STAGE, s, ja); e->prof_end(s);
+                TF_LAUNCH(e, k_json_pass1, nlb, 128, JSN_STAGE, s, ja);
                 CK(cudaMemcpyAsync(&n_nonempty, (uint32_t*)(B + o_rank) + nlines, 4, cudaMemcpyDeviceToHost, s));
                 if (nslots) {
                     // text heaps (the staged batch is device resident, in_arena is free)
@@ -1536,7 +1527,7 @@ int tfgpu_parse_json(tfgpu_engine* e, int plan_id, const char* opts_json, const 
                                    e->in_arena, "json batch: a text column exceeds 4 GiB");
                     heap = e->in_arena.p;
                     JsnWriteArgs wa{ja, (const uint32_t*)(B + o_off), e->in_arena.p, (const uint64_t*)(B + o_base)};
-                    e->prof_begin("k_json_pass2", s); launch_k_json_pass2(nlb, 128, JSN_STAGE, s, wa); e->prof_end(s);
+                    TF_LAUNCH(e, k_json_pass2, nlb, 128, JSN_STAGE, s, wa);
                 } else CK(cudaStreamSynchronize(s));
             }
             // ---- the staged batch, device resident
@@ -1659,7 +1650,6 @@ int tfgpu_parse_debezium(tfgpu_engine* e, int plan_id, const char* opts_json, co
         uint8_t* B = e->csv_stage.p;
         for (size_t c = 0; c < nc; c++) { if (hc[c].w) hc[c].values = B + o_val[c]; hc[c].validity = (uint32_t*)(B + o_vld[c]); }
         Heaps h; const uint8_t* heap = nullptr;
-        e->prof_n = 0;
         if (n) {
             CK(cudaMemcpyAsync(B + o_end, msg_ends, n * 8, cudaMemcpyHostToDevice, s));
             CK(cudaMemcpyAsync(B + o_cols, hc.data(), nc * sizeof(DbzColDev), cudaMemcpyHostToDevice, s));
@@ -1672,15 +1662,14 @@ int tfgpu_parse_debezium(tfgpu_engine* e, int plan_id, const char* opts_json, co
             da.span_start = (uint32_t*)(B + o_ss); da.span_len = (uint32_t*)(B + o_sl); da.out_len = (uint32_t*)(B + o_len);
             da.kinds = B + o_kind; da.tx_id = (uint32_t*)(B + o_tx); da.lsn = (uint64_t*)(B + o_lsn); da.commit_time = (uint64_t*)(B + o_ct); da.err = B + o_err; da.errcol = B + o_ecol;
             const uint32_t nb = (uint32_t)((n + 127) / 128);
-            e->prof_begin("k_dbz_pass1", s); launch_k_dbz_pass1(nb, 128, DBZ_STAGE, s, da); e->prof_end(s);
+            TF_LAUNCH(e, k_dbz_pass1, nb, 128, DBZ_STAGE, s, da);
             if (nslots) {
                 h = size_heaps(e, (const uint32_t*)(B + o_len), n, (uint32_t)nslots, (uint32_t*)(B + o_off), (uint64_t*)(B + o_tot), (uint64_t*)(B + o_base),
                                e->in_arena, "debezium batch: a text column exceeds 4 GiB");
                 heap = e->in_arena.p;
                 DbzWriteArgs wa{da, (const uint32_t*)(B + o_off), e->in_arena.p, (const uint64_t*)(B + o_base)};
-                e->prof_begin("k_dbz_pass2", s); launch_k_dbz_pass2(nb, 128, 0, s, wa); e->prof_end(s);
+                TF_LAUNCH(e, k_dbz_pass2, nb, 128, 0, s, wa);
             }
-            CK(cudaGetLastError());
         }
         std::vector<tf_col> dev(nc);
         for (size_t c = 0; c < nc; c++) {

@@ -1,15 +1,3 @@
 // translation unit of the csv kernels
 #define TF_KERNELS_CSV
-#include <cuda_runtime.h>
 #include "kernels_csv.cuh"
-namespace tfk {
-void launch_k_csv_count_nl(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint8_t* text, uint64_t len, uint32_t* blk_cnt, const uint32_t* endbits) { k_csv_count_nl<<<grid, block, smem, s>>>(text, len, blk_cnt, endbits); }
-void launch_k_csv_line_index(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint8_t* text, uint64_t len, const uint32_t* blk_off, uint32_t* line_end, const uint32_t* endbits) { k_csv_line_index<<<grid, block, smem, s>>>(text, len, blk_off, line_end, endbits); }
-void launch_k_csv_pass1(dim3 grid, dim3 block, size_t smem, cudaStream_t s, CsvArgs a) { k_csv_pass1<<<grid, block, smem, s>>>(a); }
-void launch_k_csv_offsets(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint32_t* span_len, uint64_t nrows, uint32_t* offsets , uint64_t* col_total) { k_csv_offsets<<<grid, block, smem, s>>>(span_len, nrows, offsets, col_total); }
-void launch_k_offsets_sum(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint32_t* span_len, uint64_t nrows, uint32_t nchunks, uint64_t* chunk_sum) { k_offsets_sum<<<grid, block, smem, s>>>(span_len, nrows, nchunks, chunk_sum); }
-void launch_k_offsets_chunks(dim3 grid, dim3 block, size_t smem, cudaStream_t s, uint64_t* chunk_sum, uint32_t nchunks, uint64_t* col_total) { k_offsets_chunks<<<grid, block, smem, s>>>(chunk_sum, nchunks, col_total); }
-void launch_k_offsets_write(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint32_t* span_len, uint64_t nrows, uint32_t nchunks, const uint64_t* chunk_base, const uint64_t* col_total, uint32_t* offsets) { k_offsets_write<<<grid, block, smem, s>>>(span_len, nrows, nchunks, chunk_base, col_total, offsets); }
-void launch_k_csv_pass2(dim3 grid, dim3 block, size_t smem, cudaStream_t s, CsvCopyArgs a) { k_csv_pass2<<<grid, block, smem, s>>>(a); }
-void launch_k_widen_lens(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const LensSrc* src, uint64_t nrows, uint32_t* out) { k_widen_lens<<<grid, block, smem, s>>>(src, nrows, out); }
-}  // namespace tfk

@@ -1,9 +1,3 @@
 // translation unit of the dbz kernels
 #define TF_KERNELS_DBZ
-#include <cuda_runtime.h>
 #include "kernels_dbz.cuh"
-namespace tfk {
-void launch_k_dbz_pass1(dim3 grid, dim3 block, size_t smem, cudaStream_t s, DbzArgs a) { k_dbz_pass1<<<grid, block, smem, s>>>(a); }
-void launch_k_dbz_pass2(dim3 grid, dim3 block, size_t smem, cudaStream_t s, DbzWriteArgs w) { k_dbz_pass2<<<grid, block, smem, s>>>(w); }
-cudaError_t dbz_kernels_init() { return cudaFuncSetAttribute(k_dbz_pass1, cudaFuncAttributeMaxDynamicSharedMemorySize, DBZ_STAGE); }
-}  // namespace tfk

@@ -1,12 +1,3 @@
 // translation unit of the json_in kernels
 #define TF_KERNELS_JSON_IN
-#include <cuda_runtime.h>
 #include "kernels_json_in.cuh"
-namespace tfk {
-void launch_k_json_mark_msgs(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint64_t* msg_end, uint32_t nmsgs, uint32_t* bits) { k_json_mark_msgs<<<grid, block, smem, s>>>(msg_end, nmsgs, bits); }
-void launch_k_json_count_nonempty(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint8_t* text, const uint32_t* line_end, uint64_t nlines, uint32_t* blk_cnt) { k_json_count_nonempty<<<grid, block, smem, s>>>(text, line_end, nlines, blk_cnt); }
-void launch_k_json_rank(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint8_t* text, const uint32_t* line_end, uint64_t nlines, const uint32_t* blk_off, uint32_t* rank) { k_json_rank<<<grid, block, smem, s>>>(text, line_end, nlines, blk_off, rank); }
-void launch_k_json_msg_first(dim3 grid, dim3 block, size_t smem, cudaStream_t s, const uint64_t* msg_end, uint32_t nmsgs, const uint32_t* line_end, uint64_t nlines, const uint32_t* rank, uint32_t* msg_rank0) { k_json_msg_first<<<grid, block, smem, s>>>(msg_end, nmsgs, line_end, nlines, rank, msg_rank0); }
-void launch_k_json_pass1(dim3 grid, dim3 block, size_t smem, cudaStream_t s, JsnArgs a) { k_json_pass1<<<grid, block, smem, s>>>(a); }
-void launch_k_json_pass2(dim3 grid, dim3 block, size_t smem, cudaStream_t s, JsnWriteArgs w) { k_json_pass2<<<grid, block, smem, s>>>(w); }
-}  // namespace tfk

@@ -1,8 +1,3 @@
 // translation unit of the json_out kernels
 #define TF_KERNELS_JSON_OUT
-#include <cuda_runtime.h>
 #include "kernels_json_out.cuh"
-namespace tfk {
-void launch_k_json_sizes(dim3 grid, dim3 block, size_t smem, cudaStream_t s, JsonArgs a) { k_json_sizes<<<grid, block, smem, s>>>(a); }
-void launch_k_json_write(dim3 grid, dim3 block, size_t smem, cudaStream_t s, JsonArgs a) { k_json_write<<<grid, block, smem, s>>>(a); }
-}  // namespace tfk

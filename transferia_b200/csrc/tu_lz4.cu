@@ -1,13 +1,3 @@
 // translation unit of the lz4 kernels
 #define TF_KERNELS_LZ4
-#include <cuda_runtime.h>
 #include "kernels_lz4.cuh"
-namespace tfk {
-void launch_k_lz4_frames(dim3 grid, dim3 block, size_t smem, cudaStream_t s, Lz4Args a) { k_lz4_frames<<<grid, block, smem, s>>>(a); }
-void launch_k_frame_seal(dim3 grid, dim3 block, size_t smem, cudaStream_t s, FrameArgs a) { k_frame_seal<<<grid, block, smem, s>>>(a); }
-cudaError_t lz4_kernels_init() {
-    cudaError_t r = cudaFuncSetAttribute(k_lz4_frames, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lz_smem(LZ_MAX_FRAME).total);
-    if (r != cudaSuccess) return r;
-    return cudaFuncSetAttribute(k_frame_seal, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SEAL_SMEM);
-}
-}  // namespace tfk

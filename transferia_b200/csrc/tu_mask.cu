@@ -1,8 +1,3 @@
 // translation unit of the mask kernels
 #define TF_KERNELS_MASK
-#include <cuda_runtime.h>
 #include "kernels_mask.cuh"
-namespace tfk {
-void launch_k_mask_encode(dim3 grid, dim3 block, size_t smem, cudaStream_t s, MaskArgs a) { k_mask_encode<<<grid, block, smem, s>>>(a); }
-void launch_k_shard_ids(dim3 grid, dim3 block, size_t smem, cudaStream_t s, ShardArgs a) { k_shard_ids<<<grid, block, smem, s>>>(a); }
-}  // namespace tfk

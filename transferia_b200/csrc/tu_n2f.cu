@@ -1,8 +1,3 @@
 // translation unit of the n2f kernels
 #define TF_KERNELS_N2F
-#include <cuda_runtime.h>
 #include "kernels_n2f.cuh"
-namespace tfk {
-void launch_k_n2f_sizes(dim3 grid, dim3 block, size_t smem, cudaStream_t s, N2fArgs a) { k_n2f_sizes<<<grid, block, smem, s>>>(a); }
-void launch_k_n2f_write(dim3 grid, dim3 block, size_t smem, cudaStream_t s, N2fArgs a) { k_n2f_write<<<grid, block, smem, s>>>(a); }
-}  // namespace tfk

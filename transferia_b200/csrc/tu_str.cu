@@ -1,9 +1,3 @@
 // translation unit of the str kernels
 #define TF_KERNELS_STR
-#include <cuda_runtime.h>
 #include "kernels_str.cuh"
-namespace tfk {
-void launch_k_str_sizes(dim3 grid, dim3 block, size_t smem, cudaStream_t s, EncodeArgs a) { k_str_sizes<<<grid, block, smem, s>>>(a); }
-void launch_k_encode_str_plain(dim3 grid, dim3 block, size_t smem, cudaStream_t s, EncodeArgs a) { k_encode_str_plain<<<grid, block, smem, s>>>(a); }
-void launch_k_encode_str(dim3 grid, dim3 block, size_t smem, cudaStream_t s, EncodeArgs a) { k_encode_str<<<grid, block, smem, s>>>(a); }
-}  // namespace tfk
