@@ -138,9 +138,7 @@ __global__ void __launch_bounds__(TF_STR_THREADS) k_encode_str(EncodeArgs a) {
     const uint64_t j0 = (uint64_t)blockIdx.x * TF_STR_TILE;
     if (j0 >= n) return;
     uint64_t R; const uint32_t L = str_len(c, a.sel, j0 + threadIdx.x, n, R);
-    const bool tostr = c.out_kind == OK_TOSTR;
-    const uint8_t* s = (L != 0xffffffffu && L && !tostr) ? c.heap + c.offsets[R] : nullptr;
-    if (tostr && c.nullable && !a.columnar && L != 0xffffffffu) a.raw[c.null_off + j0 + threadIdx.x] = 0;   // "<nil>" is a value
+    if (c.nullable && !a.columnar && L != 0xffffffffu) a.raw[c.null_off + j0 + threadIdx.x] = 0;   // "<nil>" is a value
     uint32_t tot; const uint32_t ex = block_excl_scan(L != 0xffffffffu ? L + (a.columnar ? 0 : varint_len(L)) : 0u, &tot, sm);
     const uint64_t tb = a.tile_base[(size_t)c.str_slot * a.ntiles_cap + blockIdx.x];
     uint8_t* gdst = a.raw + c.out_off + tb;
@@ -153,25 +151,7 @@ __global__ void __launch_bounds__(TF_STR_THREADS) k_encode_str(EncodeArgs a) {
             while (v >= 0x80) { *o++ = (uint8_t)(v | 0x80); v >>= 7; }
             *o++ = (uint8_t)v;
         }
-        // The copy is latency bound if every byte waits for its own load, so each round issues four independent
-        // aligned word loads (16 source bytes, re-aligned with funnel shifts) before any byte is stored.
-        if (tostr) { MemSink ms; ms.p = o; fmt_value(ms, c, R); o = ms.p; }
-        uint32_t nb = tostr ? 0 : L;
-        const uint32_t sh = ((uint32_t)(uintptr_t)s & 3) * 8;
-        const uint32_t* sw = (const uint32_t*)((uintptr_t)s & ~(uintptr_t)3);
-        while (nb) {
-            const uint32_t take = nb < 16 ? nb : 16;
-            const uint32_t need = (take + (sh >> 3) + 3) >> 2;            // aligned words that hold these bytes (1..5)
-            uint32_t w0 = __ldg(sw), w1 = need > 1 ? __ldg(sw + 1) : 0, w2 = need > 2 ? __ldg(sw + 2) : 0, w3 = need > 3 ? __ldg(sw + 3) : 0, w4 = need > 4 ? __ldg(sw + 4) : 0;
-            if (sh) { w0 = __funnelshift_r(w0, w1, sh); w1 = __funnelshift_r(w1, w2, sh); w2 = __funnelshift_r(w2, w3, sh); w3 = __funnelshift_r(w3, w4, sh); }
-            const uint32_t ww[4] = {w0, w1, w2, w3};
-#pragma unroll
-            for (int q = 0; q < 4; q++) {
-#pragma unroll
-                for (int b = 0; b < 4; b++) if ((uint32_t)(4 * q + b) < take) o[4 * q + b] = (uint8_t)(ww[q] >> (8 * b));
-            }
-            o += take; sw += 4; nb -= take;
-        }
+        MemSink ms; ms.p = o; fmt_value(ms, c, R);
     }
     if (!staged) return;
     __syncthreads();

@@ -85,14 +85,11 @@ struct tfgpu_engine {
     uint32_t frame_bytes = LZ_MAX_FRAME;
     int sm_count = 132;                 // H100 SXM; replaced by the device's count in tfgpu_engine_create
     std::vector<std::unique_ptr<PlanDev>> plans;
-    // arenas
-    DevBuf in_arena, work, raw, wire, strict_stage, lens_arena, lens_arena2, csv_text, csv_stage, json_msgs, n2f_stage, n2f_heap, off_scratch;
+    // arenas; only run_chain lays out `work` (tfgpu_measure borrows it after join_tail): the tail reads frame sizes there
+    DevBuf in_arena, work, raw, wire, strict_stage, lens_arena, lens_arena2, csv_text, csv_stage, parse_scratch, n2f_stage, n2f_heap, off_scratch;
     DState* d_state = nullptr; DCol* d_cols = nullptr; size_t d_cols_cap = 0;
     int32_t* d_call_slots = nullptr; ColRegions* d_regions = nullptr; size_t d_call_cap = 0;   // columnar mode, per call
-    // pointers into `work` for the last call
-    uint8_t *keep = nullptr, *errcode = nullptr; uint16_t* errstep = nullptr; uint32_t *blockcnt = nullptr, *blockoff = nullptr, *sel = nullptr;
-    uint32_t* tile_sum = nullptr; uint64_t* tile_base = nullptr; uint64_t* col_bytes = nullptr; uint32_t* comp_size = nullptr; uint64_t* wire_off = nullptr; unsigned long long* frame_pfx = nullptr;
-    uint64_t last_nrows = 0; bool last_has_filter = false, last_has_sharder = false; int last_wire_fmt = 0;
+    int last_wire_fmt = 0;                             // of the last chain: tfgpu_resident_stats / _fetch read its bytes
     uint8_t* pinned = nullptr; size_t pinned_cap = 0;
     // two-phase push (tfgpu_push_encode_selective): device flags of phase one, their pinned host copy, the host gather's buffers
     DevBuf err_list;                                   // fetch_errors: counter + (row, code, term) triples
@@ -100,7 +97,6 @@ struct tfgpu_engine {
     uint64_t h2d_bytes = 0;                            // bytes stage_input has copied to the device since creation
     DevBuf json_sizes, dbz_keysz, dbz_meta, dbz_old, dbz_msgsz, old_arena, part_ids;
     DevBuf defl_meta;                                  // deflate wire formats: look-back cells, chunk checksums, work counter
-    DbzEmitArgs dbz{};                                 // set by tfgpu_emit_debezium for the TF_WIRE_DEBEZIUM branch of run_chain
     unsigned long long* lz_phases = nullptr;      // debug: per-phase cycle counters of k_lz4_frames
     void* work_json_sizes(uint64_t n) { json_sizes.ensure(n * 4 + 256); return json_sizes.p; }
     // optional per-kernel CUDA-event timing of the last call that launched anything (bench roofline), kept by launch_kernel:
@@ -130,6 +126,11 @@ void join_tail(tfgpu_engine* e) {
     if (!e->tail_pending) return;
     CK(cudaStreamWaitEvent(e->stream, e->ev_tail, 0));
     e->tail_pending = false;
+}
+// the device state of the work enqueued so far on e->stream (waits for it)
+DState read_state(tfgpu_engine* e) {
+    DState st; CK(cudaMemcpyAsync(&st, e->d_state, sizeof st, cudaMemcpyDeviceToHost, e->stream)); CK(cudaStreamSynchronize(e->stream));
+    return st;
 }
 int fail(tfgpu_engine* e, int code, const std::string& msg) { if (e) e->last_error = msg; return code; }
 int cuda_fail(tfgpu_engine* e, const CudaError& c) {
@@ -275,18 +276,18 @@ void upload_plan(PlanDev& pd) {
 
 struct Sizes { uint64_t raw_bound, n_frames_max, wire_bound; uint32_t ntiles_cap, nblocks; };
 
-Sizes compute_sizes(const tfgpu_engine* e, const PlanDev& pd, const tf_batch* in, bool columnar = false, bool json = false) {
-    const tfplan::Plan& pl = pd.plan; const uint64_t n = in->nrows;
+Sizes compute_sizes(const tfgpu_engine* e, const PlanDev& pd, uint64_t n, const tf_col* cols, bool columnar, bool json) {
+    const tfplan::Plan& pl = pd.plan;
     uint64_t raw = 64 + pl.col_headers.size();
     for (int oc : pl.out_cols) {
         const size_t c = (size_t)oc;
         if (pd.col_nullable[c]) raw += n;
         bool n2f = false; for (int q : pl.n2f_cols) if ((size_t)q == c) n2f = true;       // number_to_float may lengthen literals (1e20 -> 100000000000000000000)
-        if (pd.col_out_kind[c] == OK_STR) raw += (n2f ? 6 : 1) * in->cols[c].heap_len + 5 * n;
-        else if (pd.col_out_kind[c] == OK_TOSTR) raw += (in_width(in->cols[c].type) ? 40 * n : (n2f ? 36 : 6) * in->cols[c].heap_len + 8 * n) + 5 * n;   // longest text form (RFC3339Nano / %v float / \\u00XX-escaped JSON string)
+        if (pd.col_out_kind[c] == OK_STR) raw += (n2f ? 6 : 1) * cols[c].heap_len + 5 * n;
+        else if (pd.col_out_kind[c] == OK_TOSTR) raw += (in_width(cols[c].type) ? 40 * n : (n2f ? 36 : 6) * cols[c].heap_len + 8 * n) + 5 * n;   // longest text form (RFC3339Nano / %v float / \\u00XX-escaped JSON string)
         else raw += (uint64_t)pd.col_out_w[c] * n;
         if (columnar) raw += 8 * n + 4 * (n + 1) + n / 8 + 6 * 16 + (pd.col_out_kind[c] == OK_MASK ? 64 * n : 0);   // widest value, aux, offsets, bitmap, padding
-        if (json) raw += (uint64_t)(pl.in_schema[c].name.size() + 4 + 48) * n + (in_width(in->cols[c].type) ? 0 : (n2f ? 36 : 6) * in->cols[c].heap_len);   // name, quotes, longest scalar text, escaped payload
+        if (json) raw += (uint64_t)(pl.in_schema[c].name.size() + 4 + 48) * n + (in_width(cols[c].type) ? 0 : (n2f ? 36 : 6) * cols[c].heap_len);   // name, quotes, longest scalar text, escaped payload
     }
     Sizes s;
     s.raw_bound = raw + 256;
@@ -340,8 +341,6 @@ void ensure_d_cols(tfgpu_engine* e, size_t nc) {
     CK(cudaMalloc(&e->d_cols, sizeof(DCol) * nc)); e->d_cols_cap = nc;
 }
 
-// Launch the whole fused chain on e->stream. `cols_host` holds DEVICE pointers.
-#define TF_WIRE_COLUMNAR_INTERNAL 100
 // x-extent of a (tiles, slots) grid whose kernel strides over its tiles: enough CTAs for `waves` full waves of the device
 // (resident CTAs per SM taken as 6 for the 256-thread encode kernels), never more than the tiles there can be
 uint32_t grid_cap(const tfgpu_engine* e, uint32_t tiles_upper, uint32_t nslots, uint32_t waves) {
@@ -369,20 +368,26 @@ void run_deflate(tfgpu_engine* e, const uint8_t* text, uint64_t total, bool zlib
     TF_LAUNCH(e, k_deflate_finish, 1, 1024, 0, s, da);
 }
 
-void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* dev_cols, const uint8_t* dev_kinds, int wire_fmt, const uint8_t* pre_err = nullptr) {
-    const bool columnar = wire_fmt == TF_WIRE_COLUMNAR_INTERNAL;
+// What run_chain leaves for its caller: row-error flags and `sel` (input row of every kept row; null when no row went through
+// k_filter) in e->work, valid until the next chain, and whether the plan's sharder wrote e->part_ids.
+struct ChainOut { uint8_t* errcode; uint16_t* errstep; const uint32_t* sel; bool has_sharder; };
+
+// Launches the whole fused chain over n rows on e->stream. `dev_cols` hold DEVICE pointers. out_fmt is a wire format, or 0 for the
+// Transformed rows in tf_batch layout (tfgpu_push_columns, the parsers). `dz` is the Debezium emitter's template (TF_WIRE_DEBEZIUM).
+ChainOut run_chain(tfgpu_engine* e, PlanDev& pd, uint64_t n, const tf_col* dev_cols, const uint8_t* dev_kinds, int out_fmt, const uint8_t* pre_err = nullptr, const DbzEmitArgs* dz = nullptr) {
+    const bool columnar = out_fmt == 0;
     const tfplan::Plan& pl = pd.plan;
-    const size_t nc = pl.in_schema.size(); const uint64_t n = in->nrows;
-    const int wire_base = wire_fmt == TF_WIRE_COLUMNAR_INTERNAL ? wire_fmt : (wire_fmt & 0xff);
+    const size_t nc = pl.in_schema.size();
+    const int wire_base = out_fmt & 0xff;
     const bool dbz = wire_base == TF_WIRE_DEBEZIUM;
     const bool ser = wire_base == TF_WIRE_SER_JSON || wire_base == TF_WIRE_SER_CSV || dbz;
     const bool json_rows = wire_base == TF_WIRE_CH_JSONEACHROW || ser;
     if (ser) for (size_t c = 0; c < nc; c++) if (pd.col_out_kind[c] == OK_TOSTR && pl.in_schema[c].tf == TF_ANY)
         throw tfplan::FatalError(TF_E_FATAL_UNSUPPORTED, "serializer sinks after convert_to_string on an `any` column are not handled on the device");
-    const Sizes sz = compute_sizes(e, pd, in, columnar, json_rows);
+    const Sizes sz = compute_sizes(e, pd, n, dev_cols, columnar, json_rows);
     cudaStream_t s = e->stream;
     // a pending checksum kernel may only stay in flight across a call that lays the work arena out identically
-    if (e->tail_pending && !(wire_fmt == TF_WIRE_CH_NATIVE_LZ4 && n == e->tail_nrows && (const void*)&pd == e->tail_plan && sz.n_frames_max == e->tail_nframes_max)) join_tail(e);
+    if (e->tail_pending && !(out_fmt == TF_WIRE_CH_NATIVE_LZ4 && n == e->tail_nrows && (const void*)&pd == e->tail_plan && sz.n_frames_max == e->tail_nframes_max)) join_tail(e);
     // work arena
     const size_t nslot_alloc = (size_t)(pd.n_str > 0 ? pd.n_str : 1);
     Layout W;
@@ -391,12 +396,11 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
                  o_comp = W.take(sz.n_frames_max * 4), o_wire_off = W.take(sz.n_frames_max * 8), o_pfx = W.take(sz.n_frames_max * 8), o_col_bytes = W.take(nslot_alloc * 8);
     e->work.ensure(W.total());
     uint8_t* w = e->work.p;
-    e->keep = w + o_keep; e->errcode = w + o_errcode; e->errstep = (uint16_t*)(w + o_errstep);
-    e->blockcnt = (uint32_t*)(w + o_blockcnt); e->blockoff = (uint32_t*)(w + o_blockoff); e->sel = (uint32_t*)(w + o_sel);
-    e->tile_sum = (uint32_t*)(w + o_tile_sum); e->tile_base = (uint64_t*)(w + o_tile_base);
-    e->comp_size = (uint32_t*)(w + o_comp); e->wire_off = (uint64_t*)(w + o_wire_off); e->frame_pfx = (unsigned long long*)(w + o_pfx); e->col_bytes = (uint64_t*)(w + o_col_bytes);
+    uint8_t* keep = w + o_keep; uint8_t* errcode = w + o_errcode; uint16_t* errstep = (uint16_t*)(w + o_errstep); uint32_t* blockcnt = (uint32_t*)(w + o_blockcnt); uint32_t* blockoff = (uint32_t*)(w + o_blockoff);
+    uint32_t* tile_sum = (uint32_t*)(w + o_tile_sum); uint64_t* tile_base = (uint64_t*)(w + o_tile_base); uint64_t* col_bytes = (uint64_t*)(w + o_col_bytes);
+    uint32_t* comp_size = (uint32_t*)(w + o_comp); uint64_t* wire_off = (uint64_t*)(w + o_wire_off); unsigned long long* frame_pfx = (unsigned long long*)(w + o_pfx);
     e->raw.ensure(sz.raw_bound);
-    const bool lz = wire_fmt == TF_WIRE_CH_NATIVE_LZ4;
+    const bool lz = out_fmt == TF_WIRE_CH_NATIVE_LZ4;
     if (lz) e->wire.ensure(sz.wire_bound);
     ensure_d_cols(e, nc);
     // column descriptors
@@ -459,22 +463,22 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
     }
     // sink / serializer wire formats take INSERT rows only on the device (sink_table.go:296-305 refuses the others on non-updatable
     // tables, marshal.go:92-95 and the queue serializers need OldKeys): update / delete rows that survive the chain come back as row errors
-    const bool sink_guard = dev_kinds && wire_fmt != TF_WIRE_COLUMNAR_INTERNAL && wire_base != TF_WIRE_DEBEZIUM;
+    const bool sink_guard = dev_kinds && !columnar && !dbz;
     const bool has_filter = pd.n_fsteps > 0 || pre_err || sink_guard;
-    e->last_nrows = n; e->last_has_filter = has_filter; e->last_wire_fmt = wire_fmt;
+    e->last_wire_fmt = out_fmt;
     const uint32_t nb = (uint32_t)((n + 255) / 256);
-    if (has_filter && n) {
-        FilterArgs fa{e->d_cols, dev_kinds, n, pd.d_fsteps, pd.n_fsteps, pd.d_expr_off, pd.d_terms, pd.d_blob, e->keep, e->errcode, e->errstep, e->blockcnt, e->d_state, pre_err, pre_term, sink_guard ? 1 : 0};
+    uint32_t* sel = (has_filter && n) ? (uint32_t*)(w + o_sel) : nullptr;
+    if (sel) {
+        FilterArgs fa{e->d_cols, dev_kinds, n, pd.d_fsteps, pd.n_fsteps, pd.d_expr_off, pd.d_terms, pd.d_blob, keep, errcode, errstep, blockcnt, e->d_state, pre_err, pre_term, sink_guard ? 1 : 0};
         TF_LAUNCH(e, k_filter, nb, 256, 0, s, fa);
-        TF_LAUNCH(e, k_scan_blockcnt, 1, 1024, 0, s, e->blockcnt, e->blockoff, nb, e->d_state);
-        TF_LAUNCH(e, k_compact_sel, nb, 256, 0, s, e->keep, e->blockoff, n, e->sel);
+        TF_LAUNCH(e, k_scan_blockcnt, 1, 1024, 0, s, blockcnt, blockoff, nb, e->d_state);
+        TF_LAUNCH(e, k_compact_sel, nb, 256, 0, s, keep, blockoff, n, sel);
     }
-    const uint32_t* sel = (has_filter && n) ? e->sel : nullptr;
     const uint32_t ntiles = (uint32_t)((n + TF_STR_TILE - 1) / TF_STR_TILE);
     // (the string kernels keep one CTA per tile group and exit early past the kept rows: a capped grid with a stride loop
     // makes the CTAs of the heavy columns run several groups back to back, which measured slower on the headline batch)
     const uint32_t str_gx = std::max(1u, (ntiles + TF_STR_GROUP - 1) / TF_STR_GROUP);
-    EncodeArgs ea{e->d_cols, pd.d_str_slots, sel, e->d_state, e->raw.p, e->tile_sum, e->tile_base, sz.ntiles_cap, columnar ? 1 : 0};
+    EncodeArgs ea{e->d_cols, pd.d_str_slots, sel, e->d_state, e->raw.p, tile_sum, tile_base, sz.ntiles_cap, columnar ? 1 : 0};
     if (!has_filter || !n) {
         // n_kept = nrows is set inside k_layout (has_sel = 0); k_str_sizes needs it earlier:
         DState init; std::memset(&init, 0, sizeof init); init.n_kept = n;
@@ -485,52 +489,36 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
         ShardArgs sa{e->d_cols, pd.d_shard_cols, (int)pl.shard_cols.size(), pd.d_mask_keys, sel, e->d_state, pl.shards, (uint32_t*)e->part_ids.p};
         TF_LAUNCH(e, k_shard_ids, nb, 256, 0, s, sa);
     }
-    e->last_has_sharder = pl.has_sharder;
     if (json_rows) {
         // JSONEachRow: rows sized, placed by a tile scan, then written (kernels_json_out.cuh)
         const uint32_t jt = (uint32_t)((n + TF_JSON_TILE - 1) / TF_JSON_TILE);
         JsonArgs ja{e->d_cols, ser ? (wire_base == TF_WIRE_SER_CSV ? pd.d_scsvcols : pd.d_sjcols) : pd.d_jcols, (int)pl.out_cols.size(), ser ? pd.d_snames : pd.d_jnames, pd.d_mask_keys, sel, e->d_state, e->raw.p,
-                    (uint32_t*)e->work_json_sizes(n), e->tile_sum, e->tile_base, e->col_bytes,
-                    dbz ? 3 : ser ? (wire_base == TF_WIRE_SER_JSON ? 1 : 2) : 0, (uint32_t)(((wire_fmt & TF_WIRE_F_CLOSING_NEWLINE) ? TF_SER_NL : 0) | ((wire_fmt & TF_WIRE_F_ANY_AS_STRING) ? TF_SER_AAS : 0)), e->errcode, e->errstep, DbzEmitArgs{}};
-        if (dbz) { ja.jcols = pd.d_sjcols; e->dbz_keysz.ensure(n * 4 + 256); e->dbz_msgsz.ensure(n * 28 + 256); ja.dz = e->dbz; ja.dz.key_size = (uint32_t*)e->dbz_keysz.p; ja.dz.msg_size = (uint32_t*)e->dbz_msgsz.p; }
-        if (ser && !has_filter && n) { CK(cudaMemsetAsync(e->errcode, 0, n, s)); CK(cudaMemsetAsync(e->errstep, 0, 2 * n, s)); }
+                    (uint32_t*)e->work_json_sizes(n), tile_sum, tile_base, col_bytes,
+                    dbz ? 3 : ser ? (wire_base == TF_WIRE_SER_JSON ? 1 : 2) : 0, (uint32_t)(((out_fmt & TF_WIRE_F_CLOSING_NEWLINE) ? TF_SER_NL : 0) | ((out_fmt & TF_WIRE_F_ANY_AS_STRING) ? TF_SER_AAS : 0)), errcode, errstep, DbzEmitArgs{}};
+        if (dbz) { ja.jcols = pd.d_sjcols; e->dbz_keysz.ensure(n * 4 + 256); e->dbz_msgsz.ensure(n * 28 + 256); ja.dz = *dz; ja.dz.key_size = (uint32_t*)e->dbz_keysz.p; ja.dz.msg_size = (uint32_t*)e->dbz_msgsz.p; }
+        if (ser && !has_filter && n) { CK(cudaMemsetAsync(errcode, 0, n, s)); CK(cudaMemsetAsync(errstep, 0, 2 * n, s)); }
         if (jt) TF_LAUNCH(e, k_json_sizes, jt, TF_JSON_TILE, 0, s, ja);
-        LayoutArgs lj{e->d_cols, 0, pd.d_out_cols, pd.d_str_slots, 1, e->tile_sum, e->tile_base, sz.ntiles_cap, pd.d_col_headers, pd.d_col_header_off,
-                      e->raw.p, e->d_state, n, 1, e->frame_bytes, e->col_bytes};
+        LayoutArgs lj{e->d_cols, 0, pd.d_out_cols, pd.d_str_slots, 1, tile_sum, tile_base, sz.ntiles_cap, pd.d_col_headers, pd.d_col_header_off,
+                      e->raw.p, e->d_state, n, 1, e->frame_bytes, col_bytes};
         TF_LAUNCH(e, k_layout_scan, 1, 1024, 0, s, lj);
         uint64_t json_total = 0;
         {   // row text has no useful upper bound ('f' floats reach 300+ characters): size the output from the measured total
-            CK(cudaMemcpyAsync(&json_total, e->col_bytes, 8, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
+            CK(cudaMemcpyAsync(&json_total, col_bytes, 8, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
             e->raw.ensure(json_total + 256); ja.raw = e->raw.p;
         }
         TF_LAUNCH(e, k_json_write, jt ? jt : 1, TF_JSON_TILE, 0, s, ja);
-        if (ser && (wire_fmt & (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB))) run_deflate(e, e->raw.p, n ? json_total : 0, (wire_fmt & TF_WIRE_F_ZLIB) != 0);
-        return;
+        if (ser && (out_fmt & (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB))) run_deflate(e, e->raw.p, n ? json_total : 0, (out_fmt & TF_WIRE_F_ZLIB) != 0);
+        return ChainOut{errcode, errstep, sel, pl.has_sharder};
     }
     if (pd.n_str && ntiles) TF_LAUNCH(e, k_str_sizes, dim3(str_gx, pd.n_str), TF_STR_THREADS, 0, s, ea);
-    LayoutArgs la{e->d_cols, (int)pl.out_cols.size(), pd.d_out_cols, pd.d_str_slots, pd.n_str, e->tile_sum, e->tile_base, sz.ntiles_cap, pd.d_col_headers, pd.d_col_header_off,
-                  e->raw.p, e->d_state, n, 1, e->frame_bytes, e->col_bytes};
+    LayoutArgs la{e->d_cols, (int)pl.out_cols.size(), pd.d_out_cols, pd.d_str_slots, pd.n_str, tile_sum, tile_base, sz.ntiles_cap, pd.d_col_headers, pd.d_col_header_off,
+                  e->raw.p, e->d_state, n, 1, e->frame_bytes, col_bytes};
     if (pd.n_str) TF_LAUNCH(e, k_layout_scan, pd.n_str, 1024, 0, s, la);
-    if (!columnar) {
-        TF_LAUNCH(e, k_layout_finish, 1, 256, 0, s, la);
-        if (n) {
-            // (the fixed-width streams and the String columns write disjoint parts of the block, but running them on two streams
-            // was measured slower than running them in sequence: both are latency-bound gathers that already fill the SMs)
-            if (pd.n_fixed_slots) {
-                // widest stream is 8 bytes per row: words = 2n (+1 for misalignment)
-                const uint32_t gx = grid_cap(e, (uint32_t)((2 * n + 2 + TF_FIX_TILE_WORDS - 1) / TF_FIX_TILE_WORDS), (uint32_t)pd.n_fixed_slots, 6);
-                EncodeArgs fa = ea; fa.slots = pd.d_fixed_slots;
-                TF_LAUNCH(e, k_encode_fixed, dim3(gx, pd.n_fixed_slots), 256, 0, s, fa);
-            }
-            if (pd.n_str) TF_LAUNCH(e, k_encode_str_plain, dim3(str_gx, pd.n_str), TF_STR_THREADS, 0, s, ea);
-            if (pd.n_str && pd.n_tostr) TF_LAUNCH(e, k_encode_str, dim3(ntiles, pd.n_str), TF_STR_THREADS, 0, s, ea);
-            if (pd.n_mask_cols) {
-                MaskArgs ma{e->d_cols, pd.d_mask_slots, pd.d_mask_keys, sel, e->d_state, e->raw.p, 0};
-                TF_LAUNCH(e, k_mask_encode, dim3((uint32_t)((n + 127) / 128), pd.n_mask_cols), 128, 0, s, ma);
-            }
-        }
-    } else {
-        // Transformed rows back in tf_batch layout (tfgpu_push_columns)
+    // the fixed-width slots the encode writes: the plan's for the native block; for Transformed rows a per-call list, followed by the
+    // columns whose validity bitmap is repacked
+    const int32_t* fixed_slots = pd.d_fixed_slots; uint32_t n_fixed = (uint32_t)pd.n_fixed_slots, n_valid = 0;
+    if (!columnar) TF_LAUNCH(e, k_layout_finish, 1, 256, 0, s, la);
+    else {
         const size_t no = pl.out_cols.size();
         if (e->d_call_cap < no) {
             if (e->d_call_slots) { CK(cudaFree(e->d_call_slots)); CK(cudaFree(e->d_regions)); }
@@ -544,44 +532,49 @@ void run_chain(tfgpu_engine* e, PlanDev& pd, const tf_batch* in, const tf_col* d
             if (!fresh && d.aux) fixed.push_back(oc | TF_SLOT_AUX);
             if (!fresh && d.validity) valid.push_back(oc);
         }
-        std::vector<int32_t> both(fixed); both.insert(both.end(), valid.begin(), valid.end());
-        if (!both.empty()) CK(cudaMemcpyAsync(e->d_call_slots, both.data(), both.size() * 4, cudaMemcpyHostToDevice, s));
+        fixed_slots = e->d_call_slots; n_fixed = (uint32_t)fixed.size(); n_valid = (uint32_t)valid.size();
+        fixed.insert(fixed.end(), valid.begin(), valid.end());
+        if (!fixed.empty()) CK(cudaMemcpyAsync(e->d_call_slots, fixed.data(), fixed.size() * 4, cudaMemcpyHostToDevice, s));
         TF_LAUNCH(e, k_layout_columnar, 1, 256, 0, s, la, e->d_regions);
-        if (n) {
-            if (!fixed.empty()) {
-                const uint32_t gx = grid_cap(e, (uint32_t)((2 * n + 2 + TF_FIX_TILE_WORDS - 1) / TF_FIX_TILE_WORDS), (uint32_t)fixed.size(), 6);
-                EncodeArgs fa = ea; fa.slots = e->d_call_slots;
-                TF_LAUNCH(e, k_encode_fixed, dim3(gx, (uint32_t)fixed.size()), 256, 0, s, fa);
-            }
-            if (!valid.empty()) {
-                EncodeArgs va = ea; va.slots = e->d_call_slots + fixed.size();
-                TF_LAUNCH(e, k_pack_validity, dim3((uint32_t)((n / 8 + 256) / 256), (uint32_t)valid.size()), 256, 0, s, va);
-            }
-            if (pd.n_str) TF_LAUNCH(e, k_encode_str_plain, dim3(str_gx, pd.n_str), TF_STR_THREADS, 0, s, ea);
-            if (pd.n_str && pd.n_tostr) TF_LAUNCH(e, k_encode_str, dim3(ntiles, pd.n_str), TF_STR_THREADS, 0, s, ea);
-            if (pd.n_mask_cols) {
-                MaskArgs ma{e->d_cols, pd.d_mask_slots, pd.d_mask_keys, sel, e->d_state, e->raw.p, 1};
-                TF_LAUNCH(e, k_mask_encode, dim3((uint32_t)((n + 127) / 128), pd.n_mask_cols), 128, 0, s, ma);
-            }
+    }
+    if (n) {
+        // (the fixed-width streams and the String columns write disjoint parts of the block, but running them on two streams
+        // was measured slower than running them in sequence: both are latency-bound gathers that already fill the SMs)
+        if (n_fixed) {
+            // widest stream is 8 bytes per row: words = 2n (+1 for misalignment)
+            const uint32_t gx = grid_cap(e, (uint32_t)((2 * n + 2 + TF_FIX_TILE_WORDS - 1) / TF_FIX_TILE_WORDS), n_fixed, 6);
+            EncodeArgs fa = ea; fa.slots = fixed_slots;
+            TF_LAUNCH(e, k_encode_fixed, dim3(gx, n_fixed), 256, 0, s, fa);
+        }
+        if (n_valid) {
+            EncodeArgs va = ea; va.slots = fixed_slots + n_fixed;
+            TF_LAUNCH(e, k_pack_validity, dim3((uint32_t)((n / 8 + 256) / 256), n_valid), 256, 0, s, va);
+        }
+        if (pd.n_str) TF_LAUNCH(e, k_encode_str_plain, dim3(str_gx, pd.n_str), TF_STR_THREADS, 0, s, ea);
+        if (pd.n_str && pd.n_tostr) TF_LAUNCH(e, k_encode_str, dim3(ntiles, pd.n_str), TF_STR_THREADS, 0, s, ea);
+        if (pd.n_mask_cols) {
+            MaskArgs ma{e->d_cols, pd.d_mask_slots, pd.d_mask_keys, sel, e->d_state, e->raw.p, columnar ? 1 : 0};
+            TF_LAUNCH(e, k_mask_encode, dim3((uint32_t)((n + 127) / 128), pd.n_mask_cols), 128, 0, s, ma);
         }
     }
     if (lz) {
-        Lz4Args za{e->raw.p, e->d_state, e->wire.p, e->comp_size, e->wire_off, e->frame_pfx, e->d_tail, e->frame_bytes, e->lz_phases};
+        Lz4Args za{e->raw.p, e->d_state, e->wire.p, comp_size, wire_off, frame_pfx, e->d_tail, e->frame_bytes, e->lz_phases};
         const size_t smem = lz_smem(e->frame_bytes).total;
         const uint32_t per_sm = (uint32_t)std::max<size_t>(1, std::min<size_t>(LZ_CTAS_PER_SM, (227 * 1024) / (smem + 1024)));
         const uint32_t grid = (uint32_t)std::min<uint64_t>(sz.n_frames_max, (uint64_t)e->sm_count * per_sm);
         join_tail(e);            // the previous batch's checksum kernel still reads the wire bytes and sizes this kernel overwrites
-        CK(cudaMemsetAsync(e->frame_pfx, 0, sz.n_frames_max * 8, s));
+        CK(cudaMemsetAsync(frame_pfx, 0, sz.n_frames_max * 8, s));
         // frames are compressed and written at their final wire offset by one kernel (sizes of the earlier frames by decoupled look-back)
         TF_LAUNCH(e, k_lz4_frames, grid, LZ_THREADS, smem, s, za);
         // the checksum kernel (one thread per frame: latency-bound, a few warps per SM) runs on the side stream, under the next batch
-        FrameArgs fa{e->comp_size, e->wire_off, e->wire.p, e->d_tail};
+        FrameArgs fa{comp_size, wire_off, e->wire.p, e->d_tail};
         cudaStream_t s3 = e->side_stream;
         CK(cudaEventRecord(e->ev_fork, s)); CK(cudaStreamWaitEvent(s3, e->ev_fork, 0));
         TF_LAUNCH(e, k_frame_seal, (uint32_t)((sz.n_frames_max + 31) / 32), 32, SEAL_SMEM, s3, fa);
         CK(cudaEventRecord(e->ev_tail, s3));
         e->tail_pending = true; e->tail_nrows = n; e->tail_plan = (const void*)&pd; e->tail_nframes_max = sz.n_frames_max;      // joined by whoever needs the wire bytes, or by the next batch before its LZ4
     }
+    return ChainOut{errcode, errstep, sel, pl.has_sharder};
 }
 
 }  // namespace
@@ -594,6 +587,16 @@ static bool wire_is_ser(int wire_fmt) {
            (wire_fmt & (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB)) != (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB);
 }
 static bool wire_known(int wire_fmt) { return wire_fmt == TF_WIRE_CH_NATIVE || wire_fmt == TF_WIRE_CH_NATIVE_LZ4 || wire_fmt == TF_WIRE_CH_JSONEACHROW || wire_is_ser(wire_fmt); }
+
+// The checks every batch entry point makes before its own: engine, batch and plan id (TF_E_FATAL_ARG, no message), then the batch's
+// column count and row count. Sets `pd` to the plan.
+static int check_batch(tfgpu_engine* e, int plan_id, const tf_batch* in, PlanDev*& pd) {
+    if (!e || !in || plan_id < 0 || plan_id >= (int)e->plans.size()) return TF_E_FATAL_ARG;
+    pd = e->plans[plan_id].get();
+    if (in->ncols != pd->plan.in_schema.size()) return fail(e, TF_E_FATAL_ARG, "batch column count does not match the plan schema");
+    if (in->nrows >= (1ull << 31)) return fail(e, TF_E_FATAL_ARG, "batch too large (>= 2^31 rows)");
+    return TF_OK;
+}
 
 extern "C" {
 
@@ -703,16 +706,14 @@ const char* tfgpu_plan_describe(tfgpu_engine* e, int plan_id) {
 
 static const uint8_t* stage_input(tfgpu_engine* e, const tf_batch* in, std::vector<tf_col>& dev, DevBuf* arena_opt = nullptr);
 int tfgpu_push_encode_resident(tfgpu_engine* e, int plan_id, int wire_fmt, const tf_batch* in) {
-    if (!e || !in || plan_id < 0 || plan_id >= (int)e->plans.size()) return TF_E_FATAL_ARG;
-    PlanDev& pd = *e->plans[plan_id];
-    if (!pd.plan.has_sink) return fail(e, TF_E_FATAL_CONFIG, "plan was built without a sink");
+    PlanDev* pd;
+    if (const int rc = check_batch(e, plan_id, in, pd)) return rc;
+    if (!pd->plan.has_sink) return fail(e, TF_E_FATAL_CONFIG, "plan was built without a sink");
     if (in->mem != TF_MEM_DEVICE) return fail(e, TF_E_FATAL_ARG, "tfgpu_push_encode_resident needs a TF_MEM_DEVICE batch");
-    if (in->ncols != pd.plan.in_schema.size()) return fail(e, TF_E_FATAL_ARG, "batch column count does not match the plan schema");
     if (wire_fmt != TF_WIRE_CH_NATIVE && wire_fmt != TF_WIRE_CH_NATIVE_LZ4) return fail(e, TF_E_FATAL_UNSUPPORTED, "wire format not implemented");
-    if (in->nrows >= (1ull << 31)) return fail(e, TF_E_FATAL_ARG, "batch too large (>= 2^31 rows)");
     return on_device(e, [&] {
         std::vector<tf_col> dev; const uint8_t* dev_kinds = stage_input(e, in, dev);    // device pointers pass through; TF_COL_LENS8 / 16 lengths become offsets
-        run_chain(e, pd, in, dev.data(), dev_kinds, wire_fmt);
+        run_chain(e, *pd, in->nrows, dev.data(), dev_kinds, wire_fmt);
         return TF_OK;
     });
 }
@@ -721,7 +722,7 @@ int tfgpu_resident_stats(tfgpu_engine* e, uint64_t* rows_out, uint64_t* raw_byte
     if (!e) return TF_E_FATAL_ARG;
     return on_device(e, [&] {
         join_tail(e);
-        DState st; CK(cudaMemcpyAsync(&st, e->d_state, sizeof st, cudaMemcpyDeviceToHost, e->stream)); CK(cudaStreamSynchronize(e->stream));
+        const DState st = read_state(e);
         if (rows_out) *rows_out = st.n_kept; if (raw_bytes) *raw_bytes = st.raw_total;
         if (wire_bytes) *wire_bytes = e->last_wire_fmt == TF_WIRE_CH_NATIVE_LZ4 ? st.wire_total : st.raw_total;
         if (n_errors) *n_errors = st.n_errors;
@@ -733,7 +734,7 @@ int tfgpu_resident_fetch(tfgpu_engine* e, int what, uint8_t* dst, uint64_t cap) 
     if (!e || !dst) return TF_E_FATAL_ARG;
     return on_device(e, [&] {
         join_tail(e);
-        DState st; CK(cudaMemcpyAsync(&st, e->d_state, sizeof st, cudaMemcpyDeviceToHost, e->stream)); CK(cudaStreamSynchronize(e->stream));
+        const DState st = read_state(e);
         const bool wire = what == 1 && e->last_wire_fmt == TF_WIRE_CH_NATIVE_LZ4;
         const uint64_t n = wire ? st.wire_total : st.raw_total;
         if (n > cap) return fail(e, TF_E_FATAL_ARG, "destination too small");
@@ -742,22 +743,20 @@ int tfgpu_resident_fetch(tfgpu_engine* e, int what, uint8_t* dst, uint64_t cap) 
     });
 }
 
-static void fetch_errors(tfgpu_engine* e, uint64_t n, tfgpu_result* r);
-static void finish_wire(tfgpu_engine* e, uint64_t n, int wire_fmt, tfgpu_result* r);
+static void finish_wire(tfgpu_engine* e, const ChainOut& ch, uint64_t n, int wire_fmt, tfgpu_result* r);
 
 int tfgpu_push_encode(tfgpu_engine* e, int plan_id, int wire_fmt, const tf_batch* in, tfgpu_result** out) {
-    if (!e || !in || !out || plan_id < 0 || plan_id >= (int)e->plans.size()) return TF_E_FATAL_ARG;
+    if (!out) return TF_E_FATAL_ARG;
     *out = nullptr;
-    PlanDev& pd = *e->plans[plan_id];
+    PlanDev* pd;
+    if (const int rc = check_batch(e, plan_id, in, pd)) return rc;
     if (!wire_known(wire_fmt)) return fail(e, TF_E_FATAL_UNSUPPORTED, "wire format not implemented");
-    if (!wire_is_ser(wire_fmt) && !pd.plan.has_sink) return fail(e, TF_E_FATAL_CONFIG, "plan was built without a sink");
-    if (in->ncols != pd.plan.in_schema.size()) return fail(e, TF_E_FATAL_ARG, "batch column count does not match the plan schema");
-    if (in->nrows >= (1ull << 31)) return fail(e, TF_E_FATAL_ARG, "batch too large (>= 2^31 rows)");
+    if (!wire_is_ser(wire_fmt) && !pd->plan.has_sink) return fail(e, TF_E_FATAL_CONFIG, "plan was built without a sink");
     return on_device(e, [&] {
         std::vector<tf_col> dev; const uint8_t* dev_kinds = stage_input(e, in, dev);
-        run_chain(e, pd, in, dev.data(), dev_kinds, wire_fmt);
+        const ChainOut ch = run_chain(e, *pd, in->nrows, dev.data(), dev_kinds, wire_fmt);
         auto r = std::make_unique<tfgpu_result>();
-        finish_wire(e, in->nrows, wire_fmt, r.get());
+        finish_wire(e, ch, in->nrows, wire_fmt, r.get());
         *out = r.release();
         return TF_OK;
     });
@@ -811,9 +810,9 @@ int tfgpu_push_encode_selective(tfgpu_engine* e, int plan_id, int wire_fmt, cons
         const auto t_2 = std::chrono::steady_clock::now();
         // ---- phase two: the whole chain over the kept rows
         std::vector<tf_col> dev2; const uint8_t* dev_kinds2 = stage_input(e, kept, dev2);
-        run_chain(e, pd, kept, dev2.data(), dev_kinds2, wire_fmt);
+        const ChainOut ch = run_chain(e, pd, kept->nrows, dev2.data(), dev_kinds2, wire_fmt);
         auto r = std::make_unique<tfgpu_result>();
-        finish_wire(e, kept->nrows, wire_fmt, r.get());
+        finish_wire(e, ch, kept->nrows, wire_fmt, r.get());
         r->rows_in = n;
         if (trace) {
             const auto t_3 = std::chrono::steady_clock::now();
@@ -901,10 +900,10 @@ static const uint8_t* stage_input(tfgpu_engine* e, const tf_batch* in, std::vect
     return d[nb - 1];
 }
 
-static void fetch_errors(tfgpu_engine* e, uint64_t n, tfgpu_result* r) {
+static void fetch_errors(tfgpu_engine* e, const ChainOut& ch, uint64_t n, tfgpu_result* r) {
     // only the failing rows come back: (row, code, term) triples collected on the device, sorted by row here
     cudaStream_t s = e->stream;
-    DState st; CK(cudaMemcpyAsync(&st, e->d_state, sizeof st, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
+    const DState st = read_state(e);
     uint64_t cap = std::min<uint64_t>(st.n_errors, n);
     if (!cap) return;
     std::vector<DevRowErr> got;
@@ -912,7 +911,7 @@ static void fetch_errors(tfgpu_engine* e, uint64_t n, tfgpu_result* r) {
         e->err_list.ensure(cap * sizeof(DevRowErr) + 64);
         unsigned long long* counter = (unsigned long long*)e->err_list.p; DevRowErr* list = (DevRowErr*)(e->err_list.p + 16);
         CK(cudaMemsetAsync(counter, 0, 8, s));
-        TF_LAUNCH(e, k_collect_errors, (uint32_t)((n + 255) / 256), 256, 0, s, e->errcode, e->errstep, n, list, counter, cap);
+        TF_LAUNCH(e, k_collect_errors, (uint32_t)((n + 255) / 256), 256, 0, s, ch.errcode, ch.errstep, n, list, counter, cap);
         got.resize(cap); unsigned long long found = 0;
         CK(cudaMemcpyAsync(got.data(), list, cap * sizeof(DevRowErr), cudaMemcpyDeviceToHost, s));
         CK(cudaMemcpyAsync(&found, counter, 8, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
@@ -923,9 +922,9 @@ static void fetch_errors(tfgpu_engine* e, uint64_t n, tfgpu_result* r) {
     for (const DevRowErr& g : got) r->errs.push_back(tf_rowerr{g.row, g.code, g.term});
 }
 
-static void finish_columnar(tfgpu_engine* e, PlanDev& pd, uint64_t n, tfgpu_result* r) {
+static void finish_columnar(tfgpu_engine* e, PlanDev& pd, const ChainOut& ch, uint64_t n, tfgpu_result* r) {
     cudaStream_t s = e->stream;
-    DState st; CK(cudaMemcpyAsync(&st, e->d_state, sizeof st, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
+    const DState st = read_state(e);
     r->rows_in = n; r->rows_out = st.n_kept; r->raw_len = st.raw_total;
     const size_t no = pd.plan.out_cols.size();
     std::vector<ColRegions> reg(no);
@@ -938,9 +937,9 @@ static void finish_columnar(tfgpu_engine* e, PlanDev& pd, uint64_t n, tfgpu_resu
     if (!buf) throw std::bad_alloc();
     r->owned.push_back(buf);
     if (st.raw_total) CK(cudaMemcpyAsync(buf, e->raw.p, st.raw_total, cudaMemcpyDeviceToHost, s));
-    if (e->last_has_sharder && st.n_kept) { r->part_ids.resize(st.n_kept); CK(cudaMemcpyAsync(r->part_ids.data(), e->part_ids.p, st.n_kept * 4, cudaMemcpyDeviceToHost, s)); }
+    if (ch.has_sharder && st.n_kept) { r->part_ids.resize(st.n_kept); CK(cudaMemcpyAsync(r->part_ids.data(), e->part_ids.p, st.n_kept * 4, cudaMemcpyDeviceToHost, s)); }
     CK(cudaStreamSynchronize(s));
-    if (st.n_errors) fetch_errors(e, n, r);
+    if (st.n_errors) fetch_errors(e, ch, n, r);
     r->cols.resize(no);
     for (size_t k = 0; k < no; k++) {
         tf_col& c = r->cols[k]; std::memset(&c, 0, sizeof c);
@@ -952,10 +951,10 @@ static void finish_columnar(tfgpu_engine* e, PlanDev& pd, uint64_t n, tfgpu_resu
     r->batch.nrows = st.n_kept; r->batch.ncols = (uint32_t)no; r->batch.mem = TF_MEM_HOST; r->batch.cols = r->cols.data(); r->batch.kinds = nullptr;
 }
 
-static void finish_wire(tfgpu_engine* e, uint64_t n, int wire_fmt, tfgpu_result* r) {
+static void finish_wire(tfgpu_engine* e, const ChainOut& ch, uint64_t n, int wire_fmt, tfgpu_result* r) {
     cudaStream_t s = e->stream;
     join_tail(e);
-    DState st; CK(cudaMemcpyAsync(&st, e->d_state, sizeof st, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
+    const DState st = read_state(e);
     r->rows_in = n; r->rows_out = st.n_kept; r->raw_len = st.raw_total;
     const bool lz = wire_fmt == TF_WIRE_CH_NATIVE_LZ4;
     const bool wire = lz || (wire_fmt & (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB));      // compressed: the bytes are in e->wire
@@ -972,23 +971,22 @@ static void finish_wire(tfgpu_engine* e, uint64_t n, int wire_fmt, tfgpu_result*
       if ((b == TF_WIRE_SER_JSON || b == TF_WIRE_SER_CSV || b == TF_WIRE_CH_JSONEACHROW || b == TF_WIRE_DEBEZIUM) && st.n_kept) { r->row_sizes.resize(st.n_kept); CK(cudaMemcpyAsync(r->row_sizes.data(), e->json_sizes.p, st.n_kept * 4, cudaMemcpyDeviceToHost, s)); }
       if (b == TF_WIRE_DEBEZIUM && st.n_kept) { r->key_sizes.resize(st.n_kept); CK(cudaMemcpyAsync(r->key_sizes.data(), e->dbz_keysz.p, st.n_kept * 4, cudaMemcpyDeviceToHost, s));
                                                 r->msg_sizes.resize(st.n_kept * 7); CK(cudaMemcpyAsync(r->msg_sizes.data(), e->dbz_msgsz.p, st.n_kept * 28, cudaMemcpyDeviceToHost, s)); } }
-    if (e->last_has_sharder && st.n_kept) { r->part_ids.resize(st.n_kept); CK(cudaMemcpyAsync(r->part_ids.data(), e->part_ids.p, st.n_kept * 4, cudaMemcpyDeviceToHost, s)); }
-    if (st.n_errors) fetch_errors(e, n, r);
+    if (ch.has_sharder && st.n_kept) { r->part_ids.resize(st.n_kept); CK(cudaMemcpyAsync(r->part_ids.data(), e->part_ids.p, st.n_kept * 4, cudaMemcpyDeviceToHost, s)); }
+    if (st.n_errors) fetch_errors(e, ch, n, r);
     CK(cudaStreamSynchronize(s));
 }
 
 // TransformerResult{Transformed, Errors}: the kept rows come back columnar in host memory owned by the result.
 int tfgpu_push_columns(tfgpu_engine* e, int plan_id, const tf_batch* in, tfgpu_result** out) {
-    if (!e || !in || !out || plan_id < 0 || plan_id >= (int)e->plans.size()) return TF_E_FATAL_ARG;
+    if (!out) return TF_E_FATAL_ARG;
     *out = nullptr;
-    PlanDev& pd = *e->plans[plan_id];
-    if (in->ncols != pd.plan.in_schema.size()) return fail(e, TF_E_FATAL_ARG, "batch column count does not match the plan schema");
-    if (in->nrows >= (1ull << 31)) return fail(e, TF_E_FATAL_ARG, "batch too large (>= 2^31 rows)");
+    PlanDev* pd;
+    if (const int rc = check_batch(e, plan_id, in, pd)) return rc;
     return on_device(e, [&] {
         std::vector<tf_col> dev; const uint8_t* dev_kinds = stage_input(e, in, dev);
-        run_chain(e, pd, in, dev.data(), dev_kinds, TF_WIRE_COLUMNAR_INTERNAL);
+        const ChainOut ch = run_chain(e, *pd, in->nrows, dev.data(), dev_kinds, 0);
         auto r = std::make_unique<tfgpu_result>();
-        finish_columnar(e, pd, in->nrows, r.get());
+        finish_columnar(e, *pd, ch, in->nrows, r.get());
         *out = r.release();
         return TF_OK;
     });
@@ -1123,18 +1121,17 @@ int tfgpu_emit_debezium(tfgpu_engine* e, int plan_id, const char* opts_json, con
 }
 
 int tfgpu_emit_debezium_crud(tfgpu_engine* e, int plan_id, const char* opts_json, const tf_batch* in, const tf_old_keys* old, const tf_row_meta* meta, tfgpu_result** out) {
-    if (!e || !in || !out || !opts_json || plan_id < 0 || plan_id >= (int)e->plans.size()) return TF_E_FATAL_ARG;
+    if (!out || !opts_json) return TF_E_FATAL_ARG;
     *out = nullptr;
-    PlanDev& pd = *e->plans[plan_id];
-    if (in->ncols != pd.plan.in_schema.size()) return fail(e, TF_E_FATAL_ARG, "batch column count does not match the plan schema");
-    if (in->nrows >= (1ull << 31)) return fail(e, TF_E_FATAL_ARG, "batch too large (>= 2^31 rows)");
+    PlanDev* pd;
+    if (const int rc = check_batch(e, plan_id, in, pd)) return rc;
     return on_device(e, [&] {
         const uint64_t n = in->nrows;
         cudaStream_t s = e->stream;
         const tfj::ValuePtr ov = parse_opts_json(opts_json);
-        dbz_build_template(pd, opts_json, *ov);
+        dbz_build_template(*pd, opts_json, *ov);
         std::vector<tf_col> dev; const uint8_t* dev_kinds = stage_input(e, in, dev);
-        e->dbz = pd.dbz;
+        DbzEmitArgs dz = pd->dbz;
         uint64_t gt_len = 0;
         if (meta && in->mem == TF_MEM_HOST && meta->txid_offsets && meta->txid_heap) gt_len = meta->txid_offsets[n];
         Layout L(16);
@@ -1143,23 +1140,23 @@ int tfgpu_emit_debezium_crud(tfgpu_engine* e, int plan_id, const char* opts_json
         uint8_t* M = e->dbz_meta.p;
         if (meta) {
             if (in->mem == TF_MEM_HOST) {
-                if (meta->id && n) { CK(cudaMemcpyAsync(M + o_id, meta->id, n * 4, cudaMemcpyHostToDevice, s)); e->dbz.id = (const uint32_t*)(M + o_id); }
-                if (meta->lsn && n) { CK(cudaMemcpyAsync(M + o_lsn, meta->lsn, n * 8, cudaMemcpyHostToDevice, s)); e->dbz.lsn = (const uint64_t*)(M + o_lsn); }
-                if (meta->commit_time && n) { CK(cudaMemcpyAsync(M + o_ct, meta->commit_time, n * 8, cudaMemcpyHostToDevice, s)); e->dbz.ct = (const uint64_t*)(M + o_ct); }
+                if (meta->id && n) { CK(cudaMemcpyAsync(M + o_id, meta->id, n * 4, cudaMemcpyHostToDevice, s)); dz.id = (const uint32_t*)(M + o_id); }
+                if (meta->lsn && n) { CK(cudaMemcpyAsync(M + o_lsn, meta->lsn, n * 8, cudaMemcpyHostToDevice, s)); dz.lsn = (const uint64_t*)(M + o_lsn); }
+                if (meta->commit_time && n) { CK(cudaMemcpyAsync(M + o_ct, meta->commit_time, n * 8, cudaMemcpyHostToDevice, s)); dz.ct = (const uint64_t*)(M + o_ct); }
                 if (meta->txid_offsets && meta->txid_heap && n) {
-                    CK(cudaMemcpyAsync(M + o_off, meta->txid_offsets, (n + 1) * 4, cudaMemcpyHostToDevice, s)); e->dbz.gt_off = (const uint32_t*)(M + o_off);
+                    CK(cudaMemcpyAsync(M + o_off, meta->txid_offsets, (n + 1) * 4, cudaMemcpyHostToDevice, s)); dz.gt_off = (const uint32_t*)(M + o_off);
                     if (gt_len) CK(cudaMemcpyAsync(M + o_heap, meta->txid_heap, gt_len, cudaMemcpyHostToDevice, s));
-                    e->dbz.gt_heap = M + o_heap;
+                    dz.gt_heap = M + o_heap;
                 }
-            } else { e->dbz.id = meta->id; e->dbz.lsn = meta->lsn; e->dbz.ct = meta->commit_time; e->dbz.gt_off = meta->txid_offsets; e->dbz.gt_heap = meta->txid_heap; }
+            } else { dz.id = meta->id; dz.lsn = meta->lsn; dz.ct = meta->commit_time; dz.gt_off = meta->txid_offsets; dz.gt_heap = meta->txid_heap; }
         }
         // update / delete events: kinds + OldKeys (as a second set of typed columns) reach the row writer
         {
-            const tfplan::Plan& pl = pd.plan; const size_t nc = pl.in_schema.size();
-            e->dbz.kinds = dev_kinds; e->dbz.snapshot = ov->get_bool("snapshot") ? 1 : 0; e->dbz.mysql_src = ov->get_str("source_type") == "mysql" ? 1 : 0;
-            const tfj::Value* tv = ov->get("tombstones_on_delete"); e->dbz.tombstones = (tv && tv->kind == tfj::Value::Bool && !tv->b) ? 0 : 1;      // tombstones.on.delete, default true
+            const tfplan::Plan& pl = pd->plan; const size_t nc = pl.in_schema.size();
+            dz.kinds = dev_kinds; dz.snapshot = ov->get_bool("snapshot") ? 1 : 0; dz.mysql_src = ov->get_str("source_type") == "mysql" ? 1 : 0;
+            const tfj::Value* tv = ov->get("tombstones_on_delete"); dz.tombstones = (tv && tv->kind == tfj::Value::Bool && !tv->b) ? 0 : 1;      // tombstones.on.delete, default true
             int npk = 0; for (const auto& c : pl.out_schema) if (c.key) npk++;
-            e->dbz.n_pkeys = npk; e->dbz.old_cols = nullptr; e->dbz.old_present = nullptr; e->dbz.old_has = nullptr; e->dbz.n_old_present = 0;
+            dz.n_pkeys = npk;
             if (old && old->values) {
                 if (old->values->ncols != nc || old->values->nrows != n || old->values->mem != in->mem) return fail(e, TF_E_FATAL_ARG, "old keys: same shape and memory space as the batch expected");
                 if (!pl.masks.empty() || !pl.todt_cols.empty() || !pl.tostr_cols.empty() || !pl.n2f_cols.empty()) return fail(e, TF_E_FATAL_UNSUPPORTED, "update / delete events after a transformer that rewrites values are emitted by the Go emitter");
@@ -1177,17 +1174,17 @@ int tfgpu_emit_debezium_crud(tfgpu_engine* e, int plan_id, const char* opts_json
                 e->dbz_old.ensure(O.total() + 256);
                 CK(cudaMemcpyAsync(e->dbz_old.p + o_oc, oc.data(), nc * sizeof(DCol), cudaMemcpyHostToDevice, s));
                 CK(cudaMemcpyAsync(e->dbz_old.p + o_pr, present.data(), nc, cudaMemcpyHostToDevice, s));
-                e->dbz.old_cols = (const DCol*)(e->dbz_old.p + o_oc); e->dbz.old_present = e->dbz_old.p + o_pr; e->dbz.n_old_present = np;
+                dz.old_cols = (const DCol*)(e->dbz_old.p + o_oc); dz.old_present = e->dbz_old.p + o_pr; dz.n_old_present = np;
                 if (old->row_has && n) {
-                    if (in->mem == TF_MEM_HOST) { CK(cudaMemcpyAsync(e->dbz_old.p + o_has, old->row_has, n, cudaMemcpyHostToDevice, s)); e->dbz.old_has = e->dbz_old.p + o_has; }
-                    else e->dbz.old_has = old->row_has;
+                    if (in->mem == TF_MEM_HOST) { CK(cudaMemcpyAsync(e->dbz_old.p + o_has, old->row_has, n, cudaMemcpyHostToDevice, s)); dz.old_has = e->dbz_old.p + o_has; }
+                    else dz.old_has = old->row_has;
                 }
                 CK(cudaStreamSynchronize(s));      // oc / present are stack vectors
             }
         }
-        run_chain(e, pd, in, dev.data(), dev_kinds, TF_WIRE_DEBEZIUM, nullptr);
+        const ChainOut ch = run_chain(e, *pd, n, dev.data(), dev_kinds, TF_WIRE_DEBEZIUM, nullptr, &dz);
         auto r = std::make_unique<tfgpu_result>();
-        finish_wire(e, n, TF_WIRE_DEBEZIUM, r.get());
+        finish_wire(e, ch, n, TF_WIRE_DEBEZIUM, r.get());
         *out = r.release();
         return TF_OK;
     });
@@ -1244,19 +1241,30 @@ const uint8_t* stage_text(tfgpu_engine* e, const uint8_t* bytes, uint64_t len, i
     return e->csv_text.p;
 }
 
-// The staged columns (device resident, nrows rows) through the chain and out as wire_fmt asks. A row error whose term the parser left
-// open (0xff) takes the column the parser recorded for its row in d_errcol.
+// Line count of `len` bytes of text: newlines per CSV_NL_BLOCK block into blk_cnt [nblk], their exclusive scan into blk_off (which
+// the line index reads). `endbits` marks the message ends that end a line too (JSON), or is null.
+uint64_t count_lines(tfgpu_engine* e, const uint8_t* text, uint64_t len, uint32_t nblk, uint32_t* blk_cnt, uint32_t* blk_off, const uint32_t* endbits) {
+    if (!nblk) return 0;
+    cudaStream_t s = e->stream;
+    CK(cudaMemsetAsync(e->d_state, 0, sizeof(DState), s));
+    TF_LAUNCH(e, k_csv_count_nl, nblk, 256, 0, s, text, len, blk_cnt, endbits);
+    TF_LAUNCH(e, k_scan_blockcnt, 1, 1024, 0, s, blk_cnt, blk_off, nblk, e->d_state);
+    return read_state(e).n_kept;
+}
+
+// The staged columns (device resident, nrows rows) through the chain and out as wire_fmt asks; `chain` receives what the chain left.
+// A row error whose term the parser left open (0xff) takes the column the parser recorded for its row in d_errcol.
 std::unique_ptr<tfgpu_result> run_staged(tfgpu_engine* e, PlanDev& pd, std::vector<tf_col>& dev, uint64_t nrows, const uint8_t* kinds,
-                                         const uint8_t* pre_err, const uint8_t* d_errcol, int wire_fmt) {
-    const tf_batch staged{nrows, (uint32_t)dev.size(), TF_MEM_DEVICE, dev.data(), nullptr};
-    run_chain(e, pd, &staged, dev.data(), kinds, wire_fmt == 0 ? TF_WIRE_COLUMNAR_INTERNAL : wire_fmt, pre_err);
+                                         const uint8_t* pre_err, const uint8_t* d_errcol, int wire_fmt, ChainOut* chain = nullptr) {
+    const ChainOut ch = run_chain(e, pd, nrows, dev.data(), kinds, wire_fmt, pre_err);
     auto r = std::make_unique<tfgpu_result>();
-    if (wire_fmt == 0) finish_columnar(e, pd, nrows, r.get()); else finish_wire(e, nrows, wire_fmt, r.get());
+    if (wire_fmt == 0) finish_columnar(e, pd, ch, nrows, r.get()); else finish_wire(e, ch, nrows, wire_fmt, r.get());
     if (d_errcol && !r->errs.empty()) {
         std::vector<uint8_t> ecol(nrows);
         CK(cudaMemcpyAsync(ecol.data(), d_errcol, nrows, cudaMemcpyDeviceToHost, e->stream)); CK(cudaStreamSynchronize(e->stream));
         for (auto& x : r->errs) if (x.term == 0xff) x.term = ecol[x.row];
     }
+    if (chain) *chain = ch;
     return r;
 }
 
@@ -1322,18 +1330,11 @@ int tfgpu_parse_csv(tfgpu_engine* e, int plan_id, const char* opts_json, const u
         const uint8_t* d_text = stage_text(e, bytes, len, mem);
         // newline index
         const uint32_t nblk = (uint32_t)((len + CSV_NL_BLOCK - 1) / CSV_NL_BLOCK);
-        uint64_t nlines = 0;
         Layout W;
         const size_t w_cnt = W.take(((size_t)nblk + 1) * 4), w_off = W.take(((size_t)nblk + 64) * 4);
-        e->work.ensure(W.total() + 256);
-        uint32_t* blk_cnt = (uint32_t*)(e->work.p + w_cnt); uint32_t* blk_off = (uint32_t*)(e->work.p + w_off);
-        if (nblk) {
-            CK(cudaMemsetAsync(e->d_state, 0, sizeof(DState), s));
-            TF_LAUNCH(e, k_csv_count_nl, nblk, 256, 0, s, d_text, len, blk_cnt, nullptr);
-            TF_LAUNCH(e, k_scan_blockcnt, 1, 1024, 0, s, blk_cnt, blk_off, nblk, e->d_state);
-            DState st; CK(cudaMemcpyAsync(&st, e->d_state, sizeof st, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
-            nlines = st.n_kept;
-        }
+        e->parse_scratch.ensure(W.total() + 256);
+        uint32_t* blk_off = (uint32_t*)(e->parse_scratch.p + w_off);
+        const uint64_t nlines = count_lines(e, d_text, len, nblk, (uint32_t*)(e->parse_scratch.p + w_cnt), blk_off, nullptr);
         const uint64_t skip = ho.skip < nlines ? ho.skip : nlines;
         const uint64_t nrows = nlines - skip;
         // staging layout
@@ -1460,21 +1461,16 @@ int tfgpu_parse_json(tfgpu_engine* e, int plan_id, const char* opts_json, const 
             Layout M;
             const size_t w_cnt = M.take(((size_t)nblk + 64) * 4), w_off = M.take(((size_t)nblk + 64) * 4), w_bits = M.take(bits_words * 4),
                          w_end = M.take((size_t)n_msgs * 8), w_moff = M.take((size_t)n_msgs * 8), w_ws = M.take((size_t)n_msgs * 8), w_wn = M.take((size_t)n_msgs * 4), w_r0 = M.take((size_t)n_msgs * 4);
-            e->json_msgs.ensure(M.total() + 256);                // message table + line-count scratch live here until the text heap is sized
-            uint8_t* W = e->json_msgs.p;
-            uint32_t* blk_cnt = (uint32_t*)(W + w_cnt); uint32_t* blk_off = (uint32_t*)(W + w_off); uint32_t* endbits = (uint32_t*)(W + w_bits);
-            uint64_t nlines = 0;
+            e->parse_scratch.ensure(M.total() + 256);            // message table + line-count scratch live here until the text heap is sized
+            uint8_t* W = e->parse_scratch.p;
+            uint32_t* blk_off = (uint32_t*)(W + w_off); uint32_t* endbits = (uint32_t*)(W + w_bits);
             if (nblk) {
-                CK(cudaMemsetAsync(e->d_state, 0, sizeof(DState), s));
                 CK(cudaMemsetAsync(endbits, 0, bits_words * 4, s));
                 CK(cudaMemcpyAsync(W + w_end, h_end.data(), (size_t)n_msgs * 8, cudaMemcpyHostToDevice, s)); CK(cudaMemcpyAsync(W + w_moff, h_off.data(), (size_t)n_msgs * 8, cudaMemcpyHostToDevice, s));
                 CK(cudaMemcpyAsync(W + w_ws, h_ws.data(), (size_t)n_msgs * 8, cudaMemcpyHostToDevice, s)); CK(cudaMemcpyAsync(W + w_wn, h_wn.data(), (size_t)n_msgs * 4, cudaMemcpyHostToDevice, s));
                 TF_LAUNCH(e, k_json_mark_msgs, (n_msgs + 255) / 256, 256, 0, s, (const uint64_t*)(W + w_end), n_msgs, endbits);
-                TF_LAUNCH(e, k_csv_count_nl, nblk, 256, 0, s, d_text, len, blk_cnt, endbits);
-                TF_LAUNCH(e, k_scan_blockcnt, 1, 1024, 0, s, blk_cnt, blk_off, nblk, e->d_state);
-                DState st; CK(cudaMemcpyAsync(&st, e->d_state, sizeof st, cudaMemcpyDeviceToHost, s)); CK(cudaStreamSynchronize(s));
-                nlines = st.n_kept;
             }
+            const uint64_t nlines = count_lines(e, d_text, len, nblk, (uint32_t*)(W + w_cnt), blk_off, endbits);
             const uint64_t nrows = nlines;
             // ---- staging layout (csv_stage arena)
             Layout L;
@@ -1677,12 +1673,13 @@ int tfgpu_parse_debezium(tfgpu_engine* e, int plan_id, const char* opts_json, co
             if (hc[c].w) d.values = hc[c].values;
             else staged_text_col(d, hc[c].slot, B + o_off, n, heap, h);
         }
-        auto r = run_staged(e, pd, dev, n, n ? B + o_kind : nullptr, n ? B + o_err : nullptr, B + o_ecol, wire_fmt);
+        ChainOut ch;
+        auto r = run_staged(e, pd, dev, n, n ? B + o_kind : nullptr, n ? B + o_err : nullptr, B + o_ecol, wire_fmt, &ch);
         if (n) {
             r->meta_kinds.resize(n); r->meta_tx.resize(n); r->meta_lsn.resize(n); r->meta_ct.resize(n); r->selection.resize(r->rows_out);
             CK(cudaMemcpyAsync(r->meta_kinds.data(), B + o_kind, n, cudaMemcpyDeviceToHost, s)); CK(cudaMemcpyAsync(r->meta_tx.data(), B + o_tx, n * 4, cudaMemcpyDeviceToHost, s));
             CK(cudaMemcpyAsync(r->meta_lsn.data(), B + o_lsn, n * 8, cudaMemcpyDeviceToHost, s)); CK(cudaMemcpyAsync(r->meta_ct.data(), B + o_ct, n * 8, cudaMemcpyDeviceToHost, s));
-            if (r->rows_out) CK(cudaMemcpyAsync(r->selection.data(), e->sel, r->rows_out * 4, cudaMemcpyDeviceToHost, s));
+            if (r->rows_out) CK(cudaMemcpyAsync(r->selection.data(), ch.sel, r->rows_out * 4, cudaMemcpyDeviceToHost, s));   // pre_err sends every row through k_filter
             CK(cudaStreamSynchronize(s));
         }
         r->consumed = len;
