@@ -193,6 +193,21 @@ typedef struct tf_rowerr {
  * The compressed bytes are not those of Go's compress/flate: the text they decode to and the framing above are what is pinned. */
 #define TF_WIRE_F_GZIP            0x400
 #define TF_WIRE_F_ZLIB            0x800
+/* The ClickHouse HTTP uploader's Content-Encoding: zstd (httpclient/http_client_impl.go:54-86): the TF_WIRE_CH_JSONEACHROW text compressed
+ * on the device into one zstd frame (RFC 8878). Only on TF_WIRE_CH_JSONEACHROW, and not with TF_WIRE_F_GZIP / TF_WIRE_F_ZLIB (any other
+ * combination is TF_E_FATAL_UNSUPPORTED). tfgpu_result_bytes / _bytes_len give the frame, tfgpu_result_raw_len the length of the text
+ * inside it; row sizes, rows, errors and part ids are those of the same call without the flag. Layout of the frame (tfgpu_zstd_prefix
+ * relies on it):
+ *   header      28 b5 2f fd | c0 (8-byte Frame_Content_Size, no single segment, no checksum, no dictionary) | 28 (Window_Size 32 KiB,
+ *               so Block_Maximum_Size 32 KiB) | Frame_Content_Size = the text length, 8 bytes little-endian: 14 bytes
+ *   blocks      the text cut into 16 KiB chunks, one block per chunk in text order (Raw_Block, RLE_Block or Compressed_Block, whichever
+ *               is smallest); Last_Block on the last one only. An empty text is one empty last Raw_Block (01 00 00). A block's matches
+ *               reach at most 16 KiB before its chunk, never before the text's start, and a block uses no state of the blocks before it
+ *               (no repeat offsets, treeless literals or Repeat_Mode tables)
+ *   no content checksum: XXH64 is one serial chain over the whole content and cannot be combined from per-chunk pieces; decoders,
+ *               ClickHouse's included, accept frames without it
+ * The compressed bytes are not those of the reference's encoder: the text they decode to and the framing above are what is pinned. */
+#define TF_WIRE_F_ZSTD            0x1000
 
 typedef struct tfgpu_engine tfgpu_engine;
 typedef struct tfgpu_result tfgpu_result;
@@ -452,6 +467,14 @@ int  tfgpu_deflate_stream_append(tfgpu_deflate_stream* s, const uint8_t* bytes, 
                                  uint64_t* written);
 int  tfgpu_deflate_stream_close(tfgpu_deflate_stream* s, uint8_t* out, uint64_t cap, uint64_t* written);
 void tfgpu_deflate_stream_free(tfgpu_deflate_stream* s);
+
+/* The INSERT line in front of a TF_WIRE_F_ZSTD result, inside the same frame (host only): the reference compresses
+ * `INSERT INTO ... FORMAT JSONEachRow\n` and the rows as one zstd frame. Writes to out a frame header whose content size is text_len plus
+ * the frame's, then `text` as Raw_Blocks of at most 32 KiB; the body to send is out[0, *written) followed by frame[14, frame_len) (the
+ * engine's frame after its fixed header, never copied). A frame whose header is not the engine's layout, or whose block headers do not
+ * walk exactly to frame_len, is refused with TF_E_FATAL_ARG, as is out too small (cap). Returns TF_OK or TF_E_FATAL_ARG. */
+int tfgpu_zstd_prefix(const uint8_t* text, uint64_t text_len, const uint8_t* frame, uint64_t frame_len, uint8_t* out, uint64_t cap,
+                      uint64_t* written);
 
 /* Number of kernel launches issued by this engine since creation (bench `gpu_launches`). */
 uint64_t tfgpu_engine_launch_count(const tfgpu_engine* e);

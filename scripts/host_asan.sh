@@ -5,8 +5,8 @@
 set -e
 ROOT=$(cd "$(dirname "$0")/.." && pwd); OUT=${1:-/tmp/tfhost_asan}; mkdir -p "$OUT"
 CSRC="$ROOT/transferia_b200/csrc"
-HOST_TUS=("$CSRC/host_rows.cu" "$CSRC/host_sink.cu" "$CSRC/host_chwire.cu" "$CSRC/host_plan.cu" "$CSRC/host_deflate.cu")
-python - "$ROOT" "$OUT" "$CSRC/host_plan.cu" "$CSRC/host_deflate.cu" <<'PY'
+HOST_TUS=("$CSRC/host_rows.cu" "$CSRC/host_sink.cu" "$CSRC/host_chwire.cu" "$CSRC/host_plan.cu" "$CSRC/host_deflate.cu" "$CSRC/host_zstd.cu")
+python - "$ROOT" "$OUT" "$CSRC/host_plan.cu" "$CSRC/host_deflate.cu" "$CSRC/host_zstd.cu" <<'PY'
 import re, sys
 root, out, host_defs = sys.argv[1], sys.argv[2], sys.argv[3:]
 hdr = re.sub(r"/\*.*?\*/", "", open(root + "/include/tfgpu.h").read(), flags=re.S)
@@ -31,6 +31,10 @@ TFGPU_LIB_PATH="$OUT/libtfhost_asan.so" LD_PRELOAD="$(gcc -print-file-name=libas
 TFGPU_LIB_PATH="$OUT/libtfhost_asan.so" LD_PRELOAD="$(gcc -print-file-name=libasan.so) $(gcc -print-file-name=libubsan.so)" \
     ASAN_OPTIONS=detect_leaks=0:halt_on_error=1 UBSAN_OPTIONS=print_stacktrace=1:halt_on_error=1 \
     python -m pytest tests/test_deflate.py -q -m "not gpu" -p no:cacheprovider -k "stream_helper"
+# the zstd prefix helper (host_zstd.cu)
+TFGPU_LIB_PATH="$OUT/libtfhost_asan.so" LD_PRELOAD="$(gcc -print-file-name=libasan.so) $(gcc -print-file-name=libubsan.so)" \
+    ASAN_OPTIONS=detect_leaks=0:halt_on_error=1 UBSAN_OPTIONS=print_stacktrace=1:halt_on_error=1 \
+    python -m pytest tests/test_zstd.py -q -m "not gpu" -p no:cacheprovider -k "prefix"
 # the queue serializer batchers (host_plan.cu)
 TFGPU_LIB_PATH="$OUT/libtfhost_asan.so" LD_PRELOAD="$(gcc -print-file-name=libasan.so) $(gcc -print-file-name=libubsan.so)" \
     ASAN_OPTIONS=detect_leaks=0:halt_on_error=1 UBSAN_OPTIONS=print_stacktrace=1:halt_on_error=1 \

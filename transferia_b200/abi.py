@@ -103,6 +103,7 @@ TF_COL_LENS8, TF_COL_LENS16 = 1, 2
 TF_WIRE_SER_JSON, TF_WIRE_SER_CSV = 4, 5
 TF_WIRE_F_CLOSING_NEWLINE, TF_WIRE_F_ANY_AS_STRING = 0x100, 0x200
 TF_WIRE_F_GZIP, TF_WIRE_F_ZLIB = 0x400, 0x800     # the row text as one gzip member / zlib stream (include/tfgpu.h)
+TF_WIRE_F_ZSTD = 0x1000                            # the JSONEachRow text as one zstd frame (include/tfgpu.h)
 TF_WIRE_DEBEZIUM = 6
 TF_ROWERR_CSV_BAD_FLOAT, TF_ROWERR_CSV_UNSUPPORTED, TF_ROWERR_CSV_DQ_DISABLED, TF_ROWERR_CSV_QUOTING_DISABLED = 22, 23, 24, 25
 TF_ROWERR_N2F_HOST = 52
@@ -389,6 +390,7 @@ TFGPU_H_PROTOTYPES = {
     "tfgpu_deflate_stream_append": (_i, [_v, _v, _u64, _u64, _v, _u64, _P(_u64)]),
     "tfgpu_deflate_stream_close": (_i, [_v, _v, _u64, _P(_u64)]),
     "tfgpu_deflate_stream_free": (None, [_v]),
+    "tfgpu_zstd_prefix": (_i, [_v, _u64, _v, _u64, _v, _u64, _P(_u64)]),
     "tfgpu_engine_launch_count": (_u64, [_v]),
     "tfgpu_profile_enable": (_i, [_v, _i]),
     "tfgpu_profile_read": (_s, [_v]),

@@ -137,7 +137,8 @@ struct tfgpu_sink {
         if (it != plans.end()) return it->second;
         TablePlan tp;
         const std::string ns = t.schema ? t.schema : "", name = t.table ? t.table : "";
-        const bool want_sink = wire_fmt == TF_WIRE_CH_NATIVE || wire_fmt == TF_WIRE_CH_NATIVE_LZ4 || wire_fmt == TF_WIRE_CH_JSONEACHROW;
+        const bool want_sink = wire_fmt == TF_WIRE_CH_NATIVE || wire_fmt == TF_WIRE_CH_NATIVE_LZ4 || wire_fmt == TF_WIRE_CH_JSONEACHROW ||
+                               wire_fmt == (TF_WIRE_CH_JSONEACHROW | TF_WIRE_F_ZSTD);
         tfplan::Plan pl;
         std::string schema_text = t.schema_json ? t.schema_json : "[]";
         if (updateable) {

@@ -99,10 +99,10 @@ __device__ __forceinline__ void df_put(uint32_t* img, uint32_t at, uint32_t v, u
     if (s + n > 32) atomicOr(&img[w + 1], v >> (32 - s));
 }
 
-#ifdef TF_KERNELS_DEFLATE
+#if defined(TF_KERNELS_DEFLATE) || defined(TF_KERNELS_ZSTD)
 // Code lengths of a minimum-redundancy code limited to maxbits (one thread). w[0..n) holds the weights in ascending order
 // (n >= 2) and sym[] their symbols; lens[sym] receives the lengths (the caller zeroed the others). w is overwritten.
-__device__ void df_huff_lengths(uint32_t* w, const uint16_t* sym, int n, uint32_t maxbits, uint8_t* lens) {
+static __device__ void df_huff_lengths(uint32_t* w, const uint16_t* sym, int n, uint32_t maxbits, uint8_t* lens) {
     // Moffat & Katajainen, in place: tree (parent pointers), internal node depths, leaf depths
     w[0] += w[1];
     int root = 0, leaf = 2;
@@ -137,29 +137,22 @@ __device__ void df_huff_lengths(uint32_t* w, const uint16_t* sym, int n, uint32_
     int i = n - 1;
     for (uint32_t l = 1; l <= maxbits; l++) for (uint32_t k = 0; k < cnt[l]; k++) lens[sym[i--]] = (uint8_t)l;
 }
-// canonical codes (RFC 1951 §3.2.2), stored bit-reversed for the LSB-first bit stream (one thread)
-__device__ void df_codes(const uint8_t* lens, int n, uint16_t* codes) {
-    uint32_t cnt[16], next[16];
-    for (int l = 0; l < 16; l++) cnt[l] = 0;
-    for (int s = 0; s < n; s++) cnt[lens[s]]++;
-    cnt[0] = 0; uint32_t c = 0;
-    for (int l = 1; l < 16; l++) { c = (c + cnt[l - 1]) << 1; next[l] = c; }
-    for (int s = 0; s < n; s++) { const uint32_t l = lens[s]; codes[s] = l ? (uint16_t)(__brev(next[l]++) >> (32 - l)) : 0; }
-}
+#endif
 
-// Exclusive prefix of the sizes of chunks [0, f) (warp 0). Cells hold AGG | own size or INCL | inclusive prefix.
-__device__ __forceinline__ unsigned long long df_lookback(const DeflateArgs& a, uint32_t f, uint32_t lane) {
+// Exclusive prefix of the sizes of chunks [0, f) (warp 0). Cells hold AGG | own size or INCL | inclusive prefix; a wait past the
+// bound sets st->pad.
+__device__ __forceinline__ unsigned long long df_lookback(unsigned long long* pfx, DState* st, uint32_t f, uint32_t lane) {
     unsigned long long excl = 0;
     int64_t base = (int64_t)f;
     for (uint32_t spins = 0; base > 0;) {
         const int64_t j = base - 1 - (int64_t)lane;
-        const unsigned long long v = j >= 0 ? *(volatile unsigned long long*)&a.pfx[j] : DF_FLAG_INCL;
+        const unsigned long long v = j >= 0 ? *(volatile unsigned long long*)&pfx[j] : DF_FLAG_INCL;
         const uint32_t fl = (uint32_t)(v >> 62);
         const uint32_t incl = __ballot_sync(0xffffffffu, fl == 2), none = __ballot_sync(0xffffffffu, fl == 0);
         const uint32_t upto = incl ? (uint32_t)__ffs((int)incl) - 1 : 31u;
         const uint32_t need = upto == 31 ? 0xffffffffu : ((2u << upto) - 1);
         if (none & need) {       // an earlier chunk has not published yet (its CTA holds a lower ticket and is running)
-            if (++spins > (1u << 20)) { if (lane == 0) a.st->pad = 1; break; }      // a bounded wait keeps a bug from hanging the device
+            if (++spins > (1u << 20)) { if (lane == 0) st->pad = 1; break; }      // a bounded wait keeps a bug from hanging the device
             __nanosleep(100); continue;
         }
         unsigned long long part = lane <= upto ? (v & DF_VAL_MASK) : 0ull;
@@ -169,6 +162,17 @@ __device__ __forceinline__ unsigned long long df_lookback(const DeflateArgs& a, 
         if (incl) break;
     }
     return excl;
+}
+
+#ifdef TF_KERNELS_DEFLATE
+// canonical codes (RFC 1951 §3.2.2), stored bit-reversed for the LSB-first bit stream (one thread)
+__device__ void df_codes(const uint8_t* lens, int n, uint16_t* codes) {
+    uint32_t cnt[16], next[16];
+    for (int l = 0; l < 16; l++) cnt[l] = 0;
+    for (int s = 0; s < n; s++) cnt[lens[s]]++;
+    cnt[0] = 0; uint32_t c = 0;
+    for (int l = 1; l < 16; l++) { c = (c + cnt[l - 1]) << 1; next[l] = c; }
+    for (int s = 0; s < n; s++) { const uint32_t l = lens[s]; codes[s] = l ? (uint16_t)(__brev(next[l]++) >> (32 - l)) : 0; }
 }
 
 __device__ __forceinline__ uint32_t df_block_xor(uint32_t v, uint32_t* red) {
@@ -465,7 +469,7 @@ __global__ void __launch_bounds__(DF_THREADS, 2) k_deflate_chunks(DeflateArgs a)
 
         // ---- P7: look-back for the chunk's offset, then the image to its final place
         if (warp == 0) {
-            const unsigned long long excl = df_lookback(a, f, lane);
+            const unsigned long long excl = df_lookback(a.pfx, a.st, f, lane);
             if (lane == 0) { *(volatile unsigned long long*)&a.pfx[f] = DF_FLAG_INCL | (excl + nbytes); s_off = excl; }
         }
         __syncthreads();

@@ -13,6 +13,7 @@
 #include "kernels_dbz.cuh"
 #include "kernels_json_out.cuh"
 #include "kernels_deflate.cuh"
+#include "kernels_zstd.cuh"
 namespace tfk {
 struct CudaError { cudaError_t e; const char* what; };      // a failed CUDA call; `what` names the call, or the kernel of a launch
 

@@ -97,6 +97,7 @@ struct tfgpu_engine {
     uint64_t h2d_bytes = 0;                            // bytes stage_input has copied to the device since creation
     DevBuf json_sizes, dbz_keysz, dbz_meta, dbz_old, dbz_msgsz, old_arena, part_ids;
     DevBuf defl_meta;                                  // deflate wire formats: look-back cells, chunk checksums, work counter
+    DevBuf zstd_meta;                                  // TF_WIRE_F_ZSTD: look-back cells, work counter
     unsigned long long* lz_phases = nullptr;      // debug: per-phase cycle counters of k_lz4_frames
     void* work_json_sizes(uint64_t n) { json_sizes.ensure(n * 4 + 256); return json_sizes.p; }
     // optional per-kernel CUDA-event timing of the last call that launched anything (bench roofline), kept by launch_kernel:
@@ -368,6 +369,26 @@ void run_deflate(tfgpu_engine* e, const uint8_t* text, uint64_t total, bool zlib
     TF_LAUNCH(e, k_deflate_finish, 1, 1024, 0, s, da);
 }
 
+// zstd of `total` bytes of row text into e->wire as one frame (kernels_zstd.cuh); DState.wire_total receives its length. The total is
+// the one the host already read to size the text, so this adds no host sync.
+void run_zstd(tfgpu_engine* e, const uint8_t* text, uint64_t total) {
+    cudaStream_t s = e->stream;
+    const uint64_t nch = (total + ZS_CHUNK - 1) / ZS_CHUNK;
+    if (nch >= (1ull << 32)) throw tfplan::FatalError(TF_E_FATAL_ARG, "row text too large to compress in one call");
+    e->wire.ensure(total + nch * 3 + 64);          // every block at most a Raw_Block, plus the header (or the one empty block)
+    Layout L;
+    const size_t o_pfx = L.take(nch * 8), o_ticket = L.take(4);
+    e->zstd_meta.ensure(L.total());
+    uint8_t* M = e->zstd_meta.p;
+    CK(cudaMemsetAsync(M + o_pfx, 0, nch * 8, s)); CK(cudaMemsetAsync(M + o_ticket, 0, 4, s));
+    ZstdArgs za{text, total, e->wire.p, (unsigned long long*)(M + o_pfx), (uint32_t*)(M + o_ticket), (uint32_t)nch, e->d_state};
+    if (nch) {
+        const uint32_t grid = (uint32_t)std::min<uint64_t>(nch, (uint64_t)e->sm_count);     // one CTA of ~150 KiB per SM
+        TF_LAUNCH(e, k_zstd_chunks, grid, ZS_THREADS, zs_smem().total, s, za);
+    }
+    TF_LAUNCH(e, k_zstd_finish, 1, 32, 0, s, za);
+}
+
 // What run_chain leaves for its caller: row-error flags and `sel` (input row of every kept row; null when no row went through
 // k_filter) in e->work, valid until the next chain, and whether the plan's sharder wrote e->part_ids.
 struct ChainOut { uint8_t* errcode; uint16_t* errstep; const uint32_t* sel; bool has_sharder; };
@@ -508,6 +529,7 @@ ChainOut run_chain(tfgpu_engine* e, PlanDev& pd, uint64_t n, const tf_col* dev_c
         }
         TF_LAUNCH(e, k_json_write, jt ? jt : 1, TF_JSON_TILE, 0, s, ja);
         if (ser && (out_fmt & (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB))) run_deflate(e, e->raw.p, n ? json_total : 0, (out_fmt & TF_WIRE_F_ZLIB) != 0);
+        if (out_fmt & TF_WIRE_F_ZSTD) run_zstd(e, e->raw.p, n ? json_total : 0);
         return ChainOut{errcode, errstep, sel, pl.has_sharder};
     }
     if (pd.n_str && ntiles) TF_LAUNCH(e, k_str_sizes, dim3(str_gx, pd.n_str), TF_STR_THREADS, 0, s, ea);
@@ -586,7 +608,10 @@ static bool wire_is_ser(int wire_fmt) {
     return (b == TF_WIRE_SER_JSON || b == TF_WIRE_SER_CSV) && (wire_fmt & ~(0xff | TF_WIRE_F_CLOSING_NEWLINE | TF_WIRE_F_ANY_AS_STRING | TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB)) == 0 &&
            (wire_fmt & (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB)) != (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB);
 }
-static bool wire_known(int wire_fmt) { return wire_fmt == TF_WIRE_CH_NATIVE || wire_fmt == TF_WIRE_CH_NATIVE_LZ4 || wire_fmt == TF_WIRE_CH_JSONEACHROW || wire_is_ser(wire_fmt); }
+static bool wire_known(int wire_fmt) {
+    return wire_fmt == TF_WIRE_CH_NATIVE || wire_fmt == TF_WIRE_CH_NATIVE_LZ4 || wire_fmt == TF_WIRE_CH_JSONEACHROW ||
+           wire_fmt == (TF_WIRE_CH_JSONEACHROW | TF_WIRE_F_ZSTD) || wire_is_ser(wire_fmt);
+}
 
 // The checks every batch entry point makes before its own: engine, batch and plan id (TF_E_FATAL_ARG, no message), then the batch's
 // column count and row count. Sets `pd` to the plan.
@@ -631,7 +656,7 @@ int tfgpu_engine_create(const char* cfg_json, const int* device_ids, int n_devic
         // kernels whose dynamic shared memory passes the 48 KiB default
         const struct { const void* k; size_t smem; } big_smem[] = {
             {(const void*)k_lz4_frames, lz_smem(LZ_MAX_FRAME).total}, {(const void*)k_frame_seal, SEAL_SMEM},
-            {(const void*)k_dbz_pass1, DBZ_STAGE}, {(const void*)k_deflate_chunks, df_smem().total}};
+            {(const void*)k_dbz_pass1, DBZ_STAGE}, {(const void*)k_deflate_chunks, df_smem().total}, {(const void*)k_zstd_chunks, zs_smem().total}};
         for (const auto& b : big_smem) CK(cudaFuncSetAttribute(b.k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)b.smem));
     } catch (const CudaError& c) { return c.e == cudaErrorMemoryAllocation ? TF_E_RETRY_OOM : TF_E_RETRY_LAUNCH; }
     catch (const std::exception&) { return TF_E_FATAL_CONFIG; }
@@ -957,7 +982,7 @@ static void finish_wire(tfgpu_engine* e, const ChainOut& ch, uint64_t n, int wir
     const DState st = read_state(e);
     r->rows_in = n; r->rows_out = st.n_kept; r->raw_len = st.raw_total;
     const bool lz = wire_fmt == TF_WIRE_CH_NATIVE_LZ4;
-    const bool wire = lz || (wire_fmt & (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB));      // compressed: the bytes are in e->wire
+    const bool wire = lz || (wire_fmt & (TF_WIRE_F_GZIP | TF_WIRE_F_ZLIB | TF_WIRE_F_ZSTD));      // compressed: the bytes are in e->wire
     r->n_frames = lz ? st.n_frames : 0;
     r->bytes_len = wire ? st.wire_total : st.raw_total;
     if (e->pinned_cap < r->bytes_len + 64) {   // grow-only pinned landing buffer, owned by the engine

@@ -89,6 +89,17 @@ class DeflateStream:
             self._h = None
 
 
+def zstd_prefix(text: bytes, frame: bytes) -> bytes:
+    """`text` (the INSERT line) in front of a TF_WIRE_F_ZSTD result's frame, in one frame: returns the new header and the text's raw
+    blocks; the body to send is that followed by frame[14:]. EngineError when the frame is not in the engine's layout."""
+    L = load_library()
+    out = C.create_string_buffer(14 + len(text) + 3 * (len(text) // 32768 + 1)); n = C.c_uint64()
+    rc = L.tfgpu_zstd_prefix(text, len(text), frame, len(frame), out, len(out), C.byref(n))
+    if rc != 0:
+        raise EngineError(rc, "tfgpu_zstd_prefix: the frame is not in the engine's layout")
+    return out.raw[:n.value]
+
+
 def debezium_table_schema(schema_text: str):
     """The table schema the reference derives from a Kafka Connect envelope schema's `after` struct with the default receivers
     (pkg/debezium/receiver.go:46-62, receiver_engine.go:104-141, common/field_receiver_default.go:15-30): [{"name", "type", "key"}] of
